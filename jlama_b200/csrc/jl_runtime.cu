@@ -300,9 +300,9 @@ extern "C" int jl_gemm_tc(jl_ctx *ctx, int a_dtype, const void *a, int a_col_off
     } else {
         JL_CUDA_CHECK(ctx, cudaMemcpyAsync(dab, a, a_elems * 2, cudaMemcpyHostToDevice, ctx->stream));
     }
-    // view of B starting at row n0: the kernel indexes weight rows from 0
+    // view of B starting at row n0: the kernel indexes weight rows from 0 (row pitch cols/2 bytes for Q4, cols for Q8_0)
     DevTensor Bv = B;
-    Bv.data = (uint8_t *)B.data + (size_t)n0 * (B.cols / 2);
+    Bv.data = (uint8_t *)B.data + (size_t)n0 * dtype_row_bytes(B.dtype, B.cols);
     Bv.scales = B.scales + (size_t)n0 * (B.cols / 32);
     int rc = jl_launch_gemm_tc(ctx, ctx->stream, dab + a_col_off, lda, m, Bv, n, b_col_off, k, dr, n, 0, nullptr, 0);
     if (rc) return rc;
