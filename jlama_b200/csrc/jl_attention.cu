@@ -12,6 +12,7 @@
 #include "jl_common.cuh"
 #include "jl_attn_task.cuh"
 #include "jl_attn_flat.cuh"
+#include <algorithm>
 
 #define ATT_THREADS 128
 
@@ -24,21 +25,6 @@ __device__ __forceinline__ const void *kv_row_ptr(const KvLayout &kv, int sessio
     // F32 / BF16: kept in the element-count form their instantiations were register-allocated with
     const size_t elem = (((size_t)rl * 2 + which) * kv.ctx_per_page + rc) * kv.kv_len;
     return base + elem * (kv.kv_dtype == JL_F32 ? 4 : 2);
-}
-
-__device__ __forceinline__ float kv_load(const void *row, int i, int dtype) {
-    return dtype == JL_F32 ? ((const float *)row)[i] : bf16_bits_to_f32(((const uint16_t *)row)[i]);
-}
-
-__device__ __forceinline__ uint16_t f32_to_bf16_rne(float n) {
-    const uint32_t nbits = __float_as_uint(n);
-    const uint32_t s = (nbits >> 16) & 0x8000u, e = (nbits >> 16) & 0x7f80u, m = nbits & 0x7fffffu;
-    if (e != 0x7f80u) {
-        const int mshift = (int)(m >> 16), masked = (int)(m & 0xffff), cmp = masked - 0x8000;
-        const int m1 = cmp > 0 ? mshift + 1 : (cmp < 0 ? mshift : ((mshift & 1) ? mshift + 1 : mshift));
-        return (uint16_t)(s | (e + (uint32_t)m1));
-    }
-    return m != 0 ? (uint16_t)0x7fc0 : (uint16_t)(nbits >> 16);
 }
 
 // one CTA per row (position).  KVDT = JL_I8: every warp quantises whole 32-element blocks of the row; -1: F32 or BF16 at run time.
@@ -98,8 +84,9 @@ __global__ void rope_kv_append_kernel(const AttnParams p, float *q) {
 
 int jl_launch_rope_kv_append(jl_ctx *ctx, cudaStream_t s, const AttnParams &p, float *q_inplace) {
     if (p.rows <= 0) return JL_OK;
-    if (p.kv.kv_dtype == JL_I8) JL_CUDA_CHECK(ctx, jl_launch_kernel(rope_kv_append_kernel<JL_I8>, dim3(p.rows), dim3(256), 0, s, p, q_inplace));
-    else JL_CUDA_CHECK(ctx, jl_launch_kernel(rope_kv_append_kernel<>, dim3(p.rows), dim3(256), 0, s, p, q_inplace));
+    JL_CUDA_CHECK(ctx, kv_dispatch<false>(p.kv.kv_dtype, [&](auto t) {
+                      return jl_launch_kernel(rope_kv_append_kernel<decltype(t)::value>, dim3(p.rows), dim3(256), 0, s, p, q_inplace);
+                  }));
     ctx->launches++;
     return JL_OK;
 }
@@ -109,7 +96,6 @@ int jl_launch_rope_kv_append(jl_ctx *ctx, cudaStream_t s, const AttnParams &p, f
 // The range is walked in tiles of ATT_TILE positions staged in shared memory with coalesced
 // 128-bit loads (all loads of a tile in flight together), online softmax across tiles.
 #define ATT_TILE 64
-#define ATT_MAX_GROUP 8
 // KVDT = JL_I8: the I8 page rows, dequantised as they are staged; -1: F32 or BF16 at run time.
 template <int HS, int KVDT = -1>
 __global__ void __launch_bounds__(ATT_THREADS) paged_attention_kernel(const AttnParams p) {
@@ -119,11 +105,11 @@ __global__ void __launch_bounds__(ATT_THREADS) paged_attention_kernel(const Attn
     float4 *Ks = (float4 *)att_smem;                       // [ATT_TILE][C4] swizzled
     float4 *Vs = Ks + ATT_TILE * C4;                        // [ATT_TILE][C4] plain
     float *qs = (float *)(Vs + ATT_TILE * C4);              // [group][HS]
-    float *ps = qs + ATT_MAX_GROUP * HS;                    // [ATT_TILE][ATT_MAX_GROUP]
-    float *hm = ps + ATT_TILE * ATT_MAX_GROUP;              // [group] running max
-    float *hl = hm + ATT_MAX_GROUP;                         // [group] running sum
-    float *hc = hl + ATT_MAX_GROUP;                         // [group] correction of this tile
-    float *comb = hc + ATT_MAX_GROUP;                       // [G][ATT_MAX_GROUP][HS] (G>1 only)
+    float *ps = qs + MG_MAX_GROUP * HS;                    // [ATT_TILE][MG_MAX_GROUP]
+    float *hm = ps + ATT_TILE * MG_MAX_GROUP;              // [group] running max
+    float *hl = hm + MG_MAX_GROUP;                         // [group] running sum
+    float *hc = hl + MG_MAX_GROUP;                         // [group] correction of this tile
+    float *comb = hc + MG_MAX_GROUP;                       // [G][MG_MAX_GROUP][HS] (G>1 only)
 
     const int kvh = blockIdx.x, row = blockIdx.y, split = blockIdx.z;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -148,9 +134,9 @@ __global__ void __launch_bounds__(ATT_THREADS) paged_attention_kernel(const Attn
     }
     for (int i = tid; i < group * HS; i += ATT_THREADS) qs[i] = p.q[(size_t)row * p.q_ld + h0 * HS + i];
     if (tid < group) hm[tid] = -INFINITY, hl[tid] = 0.0f;
-    float acc[ATT_MAX_GROUP];
+    float acc[MG_MAX_GROUP];
 #pragma unroll
-    for (int h = 0; h < ATT_MAX_GROUP; h++) acc[h] = 0.0f;
+    for (int h = 0; h < MG_MAX_GROUP; h++) acc[h] = 0.0f;
     const int g = tid / HS, d = tid % HS;
 
     for (int tb = t0; tb < t1; tb += ATT_TILE) {
@@ -199,19 +185,19 @@ __global__ void __launch_bounds__(ATT_THREADS) paged_attention_kernel(const Attn
                 }
                 s = __fmul_rn(a, p.scale); // scale(): CausalSelfAttention.java:332
             }
-            ps[t * ATT_MAX_GROUP + h] = s;
+            ps[t * MG_MAX_GROUP + h] = s;
         }
         __syncthreads();
         // ---- online softmax: warp w owns heads w, w+4, ... (ATT_TILE == 64 -> two scores per lane) ----
         for (int h = warp; h < group; h += ATT_THREADS / 32) {
-            const float s0 = ps[lane * ATT_MAX_GROUP + h], s1 = ps[(lane + 32) * ATT_MAX_GROUP + h];
+            const float s0 = ps[lane * MG_MAX_GROUP + h], s1 = ps[(lane + 32) * MG_MAX_GROUP + h];
             const float m_old = hm[h];
             const float m_new = fmaxf(m_old, warp_max(fmaxf(s0, s1)));
             const float e0 = s0 == -INFINITY ? 0.0f : (float)exp((double)__fsub_rn(s0, m_new));
             const float e1 = s1 == -INFINITY ? 0.0f : (float)exp((double)__fsub_rn(s1, m_new));
             const float ts = warp_sum(e0 + e1);
-            ps[lane * ATT_MAX_GROUP + h] = e0;
-            ps[(lane + 32) * ATT_MAX_GROUP + h] = e1;
+            ps[lane * MG_MAX_GROUP + h] = e0;
+            ps[(lane + 32) * MG_MAX_GROUP + h] = e1;
             if (lane == 0) {
                 const float corr = m_old == -INFINITY ? 0.0f : (float)exp((double)__fsub_rn(m_old, m_new));
                 hc[h] = corr;
@@ -223,24 +209,24 @@ __global__ void __launch_bounds__(ATT_THREADS) paged_attention_kernel(const Attn
         // ---- P.V: thread (g,d) accumulates positions t = g, g+G, ... in order (saxpy :349-354) ----
         if (g < G) {
 #pragma unroll
-            for (int h = 0; h < ATT_MAX_GROUP; h++)
+            for (int h = 0; h < MG_MAX_GROUP; h++)
                 if (h < group) acc[h] *= hc[h];
             for (int t = g; t < cnt; t += G) {
                 const float v = ((const float *)Vs)[t * HS + d];
 #pragma unroll
-                for (int h = 0; h < ATT_MAX_GROUP; h++)
-                    if (h < group) acc[h] = fmaf(v, ps[t * ATT_MAX_GROUP + h], acc[h]);
+                for (int h = 0; h < MG_MAX_GROUP; h++)
+                    if (h < group) acc[h] = fmaf(v, ps[t * MG_MAX_GROUP + h], acc[h]);
             }
         }
     }
     if (G > 1) {
         __syncthreads();
         if (g < G)
-            for (int h = 0; h < group; h++) comb[(g * ATT_MAX_GROUP + h) * HS + d] = acc[h];
+            for (int h = 0; h < group; h++) comb[(g * MG_MAX_GROUP + h) * HS + d] = acc[h];
         __syncthreads();
         if (g == 0)
             for (int h = 0; h < group; h++)
-                for (int gg = 1; gg < G; gg++) acc[h] += comb[(gg * ATT_MAX_GROUP + h) * HS + d];
+                for (int gg = 1; gg < G; gg++) acc[h] += comb[(gg * MG_MAX_GROUP + h) * HS + d];
     }
     if (g == 0) {
         for (int h = 0; h < group; h++) {
@@ -276,11 +262,11 @@ __global__ void attention_merge_kernel(const AttnParams p) {
 template <int HS>
 static size_t att_smem_bytes() {
     constexpr int G = ATT_THREADS / HS;
-    return (size_t)2 * ATT_TILE * HS * 4 + (size_t)ATT_MAX_GROUP * HS * 4 + (size_t)ATT_TILE * ATT_MAX_GROUP * 4 +
-           3 * ATT_MAX_GROUP * 4 + (G > 1 ? (size_t)G * ATT_MAX_GROUP * HS * 4 : 0);
+    return (size_t)2 * ATT_TILE * HS * 4 + (size_t)MG_MAX_GROUP * HS * 4 + (size_t)ATT_TILE * MG_MAX_GROUP * 4 +
+           3 * MG_MAX_GROUP * 4 + (G > 1 ? (size_t)G * MG_MAX_GROUP * HS * 4 : 0);
 }
 template <int HS, int KVDT>
-static int launch_att_k(jl_ctx *ctx, cudaStream_t s, const AttnParams &p) {
+static int launch_att(jl_ctx *ctx, cudaStream_t s, const AttnParams &p) {
     const size_t smem = att_smem_bytes<HS>();
     static size_t configured[JL_MAX_DEVICES] = {};
     JL_CUDA_CHECK(ctx, (jl_ensure_dyn_smem(paged_attention_kernel<HS, KVDT>, ctx->device, smem, configured)));
@@ -293,50 +279,44 @@ static int launch_att_k(jl_ctx *ctx, cudaStream_t s, const AttnParams &p) {
     }
     return JL_OK;
 }
-template <int HS>
-static int launch_att(jl_ctx *ctx, cudaStream_t s, const AttnParams &p) {
-    return p.kv.kv_dtype == JL_I8 ? launch_att_k<HS, JL_I8>(ctx, s, p) : launch_att_k<HS, -1>(ctx, s, p);
-}
 
-int jl_launch_paged_attention(jl_ctx *ctx, cudaStream_t s, const AttnParams &p, int max_pos) {
+int jl_launch_paged_attention(jl_ctx *ctx, cudaStream_t s, const AttnParams &p) {
     if (p.rows <= 0) return JL_OK;
-    (void)max_pos;
-    if (p.heads % p.kv_heads || p.heads / p.kv_heads > ATT_MAX_GROUP)
+    if (p.heads % p.kv_heads || p.heads / p.kv_heads > MG_MAX_GROUP)
         return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "attention: head group size %d/%d unsupported", p.heads, p.kv_heads);
     if (p.splits > 1 && !p.ws) return jl_set_error(ctx, JL_ERR_INVALID, "attention: split workspace missing");
-    switch (p.head_size) {
-        case 32: return launch_att<32>(ctx, s, p);
-        case 64: return launch_att<64>(ctx, s, p);
-        case 128: return launch_att<128>(ctx, s, p);
-    }
-    return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "attention: head_size %d (supported: 32, 64, 128)", p.head_size);
+    return kv_dispatch<false>(p.kv.kv_dtype, [&](auto t) {
+        constexpr int KVDT = decltype(t)::value;
+        switch (p.head_size) {
+            case 32: return launch_att<32, KVDT>(ctx, s, p);
+            case 64: return launch_att<64, KVDT>(ctx, s, p);
+            case 128: return launch_att<128, KVDT>(ctx, s, p);
+        }
+        return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "attention: head_size %d (supported: 32, 64, 128)", p.head_size);
+    });
 }
 
-// ---- fused decode attention: RoPE + KV append + scores + softmax + P.V in ONE kernel -------------------------------------
-// For decode steps every row is a different session, so a (row, kv head, split) task can append the row's own
-// K/V and attend in the same kernel (no separate rope_kv_append launch).  grid = (kv_heads, rows, splits).
-#define FDA_THREADS 256
-template <int HS, int KVDT>
-__global__ void __launch_bounds__(FDA_THREADS) fused_decode_attention_kernel(const AttnTask t, const int layer,
-                                                                              unsigned *done_cnt, unsigned long long *trace) {
-    ktrace_begin(trace, 0xA00u | (unsigned long long)t.splits << 16);
-    ktrace_mid(trace);
-    extern __shared__ __align__(16) unsigned char fda_smem[];
+// ---- stand-alone decode attention: RoPE + KV append + scores + softmax + P.V in ONE kernel ----------------------------------
+// For decode steps every row is a different session, so a (row, kv head, split) task can append the row's own K/V and attend in
+// the same kernel (no separate rope_kv_append launch).  grid = (kv_heads, rows, splits).  The last of the `splits` CTAs of a
+// (row, kv head) to arrive merges their partials (decode_attention_epilogue).  done_cnt: the arrival counters (zero before the first
+// launch, left zero).
+template <int HS, int NT>
+__device__ __forceinline__ void decode_attention_epilogue(const AttnParams &p, int m, int kvh, unsigned *done_cnt, unsigned long long *trace,
+                                                          unsigned char *smem) {
     __shared__ int s_last;
-    const int kvh = blockIdx.x, m = blockIdx.y, split = blockIdx.z;
-    attention_task<HS, FDA_THREADS, KVDT>(t, layer, m, kvh, split, fda_smem);
-    if (t.splits > 1) {
+    if (p.splits > 1) {
         __syncthreads();
         if (threadIdx.x == 0) {
             __threadfence();
-            unsigned *c = &done_cnt[m * t.kv_heads + kvh];
+            unsigned *c = &done_cnt[m * p.kv_heads + kvh];
             const unsigned old = atomicAdd(c, 1u);
-            s_last = (old == (unsigned)t.splits - 1);
+            s_last = (old == (unsigned)p.splits - 1);
             if (s_last) *c = 0; // ready for the next launch
             __threadfence();
         }
         __syncthreads();
-        if (s_last) attention_merge<HS, FDA_THREADS>(t, m, kvh, fda_smem);
+        if (s_last) attention_merge<HS, NT>(p, m, kvh, smem);
     }
     if (trace) {
         __syncthreads();
@@ -344,75 +324,48 @@ __global__ void __launch_bounds__(FDA_THREADS) fused_decode_attention_kernel(con
     }
 }
 
+// the tiled task (jl_attn_task.cuh)
+#define FDA_THREADS 256
 template <int HS, int KVDT>
-static int launch_fda_k(jl_ctx *ctx, cudaStream_t s, const AttnTask &t, int layer, int rows, unsigned *done_cnt) {
-    const size_t smem = attention_task_smem<HS, FDA_THREADS>();
-    static size_t configured[JL_MAX_DEVICES] = {};
-    JL_CUDA_CHECK(ctx, (jl_ensure_dyn_smem(fused_decode_attention_kernel<HS, KVDT>, ctx->device, smem, configured)));
-    unsigned long long *trace = jl_ktrace_slot(ctx);
-    JL_CUDA_CHECK(ctx, jl_launch_kernel(fused_decode_attention_kernel<HS, KVDT>, dim3(t.kv_heads, rows, t.splits), dim3(FDA_THREADS), smem,
-                                        s, t, layer, done_cnt, trace));
-    ctx->launches++;
-    return JL_OK;
-}
-
-template <int HS>
-static int launch_fda(jl_ctx *ctx, cudaStream_t s, const AttnTask &t, int layer, int rows, unsigned *done_cnt) {
-    if (t.kv.kv_dtype == JL_I8) return launch_fda_k<HS, JL_I8>(ctx, s, t, layer, rows, done_cnt);
-    if (t.kv.kv_dtype == JL_F32) return launch_fda_k<HS, JL_F32>(ctx, s, t, layer, rows, done_cnt);
-    return launch_fda_k<HS, JL_BF16>(ctx, s, t, layer, rows, done_cnt);
+__global__ void __launch_bounds__(FDA_THREADS) fused_decode_attention_kernel(const AttnParams p, unsigned *done_cnt, unsigned long long *trace) {
+    ktrace_begin(trace, 0xA00u | (unsigned long long)p.splits << 16);
+    ktrace_mid(trace);
+    extern __shared__ __align__(16) unsigned char fda_smem[];
+    const int kvh = blockIdx.x, m = blockIdx.y, split = blockIdx.z;
+    attention_task<HS, FDA_THREADS, KVDT>(p, m, kvh, split, fda_smem);
+    decode_attention_epilogue<HS, FDA_THREADS>(p, m, kvh, done_cnt, trace, fda_smem);
 }
 
 // The flat decode task (jl_attn_flat.cuh: K/V rows straight into registers, one exponential per (position, head), 4-5 CTA
-// barriers whatever the context) as its own launch: grid = (kv_heads, rows, splits).  Used for batched decode (several sessions
-// per step -- the persistent kernel covers the single-session case) whenever a split holds <= FA_MAX_POS positions and the GQA
-// group is a power of two; the tiled task above stays for everything else.
+// barriers whatever the context).  Used for batched decode (several sessions per step -- the persistent kernel covers the
+// single-session case) whenever a split holds <= FA_MAX_POS positions and the GQA group is a power of two; the tiled task above
+// stays for everything else.
 #define FFA_THREADS 512
 template <int HS, int KVDT = -1>
-__global__ void __launch_bounds__(FFA_THREADS) flat_decode_attention_kernel(const AttnTask t, const int layer, unsigned *done_cnt,
-                                                                            unsigned long long *trace) {
-    ktrace_begin(trace, 0xA00u | (unsigned long long)t.splits << 16);
+__global__ void __launch_bounds__(FFA_THREADS) flat_decode_attention_kernel(const AttnParams p, unsigned *done_cnt, unsigned long long *trace) {
+    ktrace_begin(trace, 0xA00u | (unsigned long long)p.splits << 16);
     ktrace_mid(trace);
     extern __shared__ __align__(16) unsigned char ffa_smem[];
-    __shared__ int s_last;
     const int kvh = blockIdx.x, m = blockIdx.y, split = blockIdx.z;
-    attention_flat<HS, FFA_THREADS, KVDT>(t, layer, m, kvh, split, ffa_smem, [] {});
-    if (t.splits > 1) {
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            __threadfence();
-            unsigned *c = &done_cnt[m * t.kv_heads + kvh];
-            const unsigned old = atomicAdd(c, 1u);
-            s_last = (old == (unsigned)t.splits - 1);
-            if (s_last) *c = 0; // ready for the next launch
-            __threadfence();
-        }
-        __syncthreads();
-        if (s_last) attention_merge<HS, FFA_THREADS>(t, m, kvh, ffa_smem);
-    }
-    if (trace) {
-        __syncthreads();
-        ktrace_end(trace);
-    }
+    attention_flat<HS, FFA_THREADS, KVDT>(p, m, kvh, split, ffa_smem, [] {});
+    decode_attention_epilogue<HS, FFA_THREADS>(p, m, kvh, done_cnt, trace, ffa_smem);
 }
 
-template <int HS, int KVDT>
-static int launch_ffa_k(jl_ctx *ctx, cudaStream_t s, const AttnTask &t, int layer, int rows, unsigned *done_cnt) {
-    size_t smem = attention_flat_smem<HS, FFA_THREADS>();
-    const size_t msm = attention_task_smem<HS, FFA_THREADS>(); // the merge step borrows the tiled task's layout
-    if (msm > smem) smem = msm;
+template <int HS, int KVDT, bool FLAT>
+static int launch_decode_attention(jl_ctx *ctx, cudaStream_t s, const AttnParams &p, unsigned *done_cnt) {
+    void (*kernel)(const AttnParams, unsigned *, unsigned long long *);
+    size_t smem;
+    if constexpr (FLAT) // the merge step borrows the tiled task's layout
+        kernel = flat_decode_attention_kernel<HS, KVDT>, smem = std::max(attention_flat_smem<HS, FFA_THREADS>(), attention_task_smem<HS, FFA_THREADS>());
+    else
+        kernel = fused_decode_attention_kernel<HS, KVDT>, smem = attention_task_smem<HS, FDA_THREADS>();
     static size_t configured[JL_MAX_DEVICES] = {};
-    JL_CUDA_CHECK(ctx, (jl_ensure_dyn_smem(flat_decode_attention_kernel<HS, KVDT>, ctx->device, smem, configured)));
+    JL_CUDA_CHECK(ctx, jl_ensure_dyn_smem(kernel, ctx->device, smem, configured));
     unsigned long long *trace = jl_ktrace_slot(ctx);
-    JL_CUDA_CHECK(ctx, jl_launch_kernel(flat_decode_attention_kernel<HS, KVDT>, dim3(t.kv_heads, rows, t.splits), dim3(FFA_THREADS), smem, s, t, layer,
+    JL_CUDA_CHECK(ctx, jl_launch_kernel(kernel, dim3(p.kv_heads, p.rows, p.splits), dim3(FLAT ? FFA_THREADS : FDA_THREADS), smem, s, p,
                                         done_cnt, trace));
     ctx->launches++;
     return JL_OK;
-}
-
-template <int HS>
-static int launch_ffa(jl_ctx *ctx, cudaStream_t s, const AttnTask &t, int layer, int rows, unsigned *done_cnt) {
-    return t.kv.kv_dtype == JL_I8 ? launch_ffa_k<HS, JL_I8>(ctx, s, t, layer, rows, done_cnt) : launch_ffa_k<HS, -1>(ctx, s, t, layer, rows, done_cnt);
 }
 
 // max_pos: the largest position among the rows (bounds the positions a split can hold)
@@ -430,17 +383,18 @@ int jl_launch_fused_decode_attention(jl_ctx *ctx, cudaStream_t s, const AttnPara
     if (p.rows <= 0) return JL_OK;
     if (p.heads % p.kv_heads || p.heads / p.kv_heads > MG_MAX_GROUP)
         return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "attention: head group size %d/%d unsupported", p.heads, p.kv_heads);
-    AttnTask t;
-    t.heads = p.heads, t.kv_heads = p.kv_heads, t.head_size = p.head_size, t.attn_seg = p.q_ld, t.kv_seg = p.kv_ld;
-    t.kv_head0_global = p.kv_head0_global, t.splits = p.splits, t.attn_scale = p.scale;
-    t.q = p.q, t.k = p.k, t.v = p.v, t.att = p.out, t.attn_ws = p.ws, t.rope = p.rope, t.kv = p.kv;
-    t.sessions = p.sessions, t.positions = p.positions;
     if (max_pos >= 0 && flat_decode_ok(p, max_pos))
-        return p.head_size == 64 ? launch_ffa<64>(ctx, s, t, p.layer, p.rows, done_cnt) : launch_ffa<128>(ctx, s, t, p.layer, p.rows, done_cnt);
-    switch (p.head_size) {
-        case 32: return launch_fda<32>(ctx, s, t, p.layer, p.rows, done_cnt);
-        case 64: return launch_fda<64>(ctx, s, t, p.layer, p.rows, done_cnt);
-        case 128: return launch_fda<128>(ctx, s, t, p.layer, p.rows, done_cnt);
-    }
-    return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "attention: head_size %d (supported: 32, 64, 128)", p.head_size);
+        return kv_dispatch<false>(p.kv.kv_dtype, [&](auto t) {
+            constexpr int KVDT = decltype(t)::value;
+            return p.head_size == 64 ? launch_decode_attention<64, KVDT, true>(ctx, s, p, done_cnt) : launch_decode_attention<128, KVDT, true>(ctx, s, p, done_cnt);
+        });
+    return kv_dispatch<true>(p.kv.kv_dtype, [&](auto t) {
+        constexpr int KVDT = decltype(t)::value;
+        switch (p.head_size) {
+            case 32: return launch_decode_attention<32, KVDT, false>(ctx, s, p, done_cnt);
+            case 64: return launch_decode_attention<64, KVDT, false>(ctx, s, p, done_cnt);
+            case 128: return launch_decode_attention<128, KVDT, false>(ctx, s, p, done_cnt);
+        }
+        return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "attention: head_size %d (supported: 32, 64, 128)", p.head_size);
+    });
 }

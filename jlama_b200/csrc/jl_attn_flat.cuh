@@ -32,8 +32,7 @@ __host__ __device__ constexpr size_t attention_flat_smem() {
 // KVDT = JL_I8: I8 page rows (a lane's HS / 8 dimensions lie in one block: one int8 load and one scale load per row part), and the
 // owner's append quantises one 32-element block per warp; -1: F32 or BF16 at run time.
 template <int HS, int NT, int KVDT = -1, typename Wait>
-__device__ __forceinline__ void attention_flat(const AttnTask &P, const int layer, const int m, const int kvh, const int split, unsigned char *u,
-                                               Wait wait) {
+__device__ __forceinline__ void attention_flat(const AttnParams &P, const int m, const int kvh, const int split, unsigned char *u, Wait wait) {
     constexpr int NW = NT / 32;
     constexpr int DPL = HS / 8;  // dims per lane
     constexpr int NF = DPL / 4;  // float4 per lane per row
@@ -57,7 +56,7 @@ __device__ __forceinline__ void attention_flat(const AttnTask &P, const int laye
     const int nsteps = (cnt + 3) / 4;
     const int h0 = kvh * group, xoff = kvh * HS, dt = KVDT >= 0 ? KVDT : P.kv.kv_dtype;
     const bool owner = pos >= t0 && pos < t1;
-    const int lpage = layer / P.kv.layers_per_page, rlayer = layer - lpage * P.kv.layers_per_page;
+    const int lpage = P.layer / P.kv.layers_per_page, rlayer = P.layer - lpage * P.kv.layers_per_page;
     const size_t v_off = kv_rows_bytes<KVDT>(dt, P.kv.kv_len, P.kv.ctx_per_page);
     const size_t layer_off = kv_rows_bytes<KVDT>(dt, P.kv.kv_len, (size_t)rlayer * 2 * P.kv.ctx_per_page);
     char *const *ptab = (char *const *)P.kv.page_table + ((size_t)session * P.kv.n_layer_pages + lpage) * P.kv.n_ctx_pages;
@@ -111,7 +110,7 @@ __device__ __forceinline__ void attention_flat(const AttnTask &P, const int laye
     for (int idx = tid; idx < group * hp; idx += NT) {
         const int h = idx / hp, j = idx - h * hp;
         const float2 f = __ldg((const float2 *)P.rope + poffset + (size_t)(P.kv_head0_global + kvh) * HS + j);
-        const float *qr = P.q + (size_t)m * P.attn_seg + (h0 + h) * HS;
+        const float *qr = P.q + (size_t)m * P.q_ld + (h0 + h) * HS;
         const float q0 = __ldcg(qr + j), q1 = __ldcg(qr + j + hp);
         qs[h * HS + j] = __fsub_rn(__fmul_rn(q0, f.x), __fmul_rn(q1, f.y));
         qs[h * HS + j + hp] = __fadd_rn(__fmul_rn(q0, f.y), __fmul_rn(q1, f.x));
@@ -121,15 +120,15 @@ __device__ __forceinline__ void attention_flat(const AttnTask &P, const int laye
         const int blk = NW - 1 - warp;
         if (owner && blk < HS / 32) {
             const int j = blk * 32 + lane;
-            const float r = rope_key_elem(P.k + (size_t)m * P.kv_seg + xoff, (const float2 *)P.rope + poffset + (size_t)(P.kv_head0_global + kvh) * HS, j, hp);
+            const float r = rope_key_elem(P.k + (size_t)m * P.kv_ld + xoff, (const float2 *)P.rope + poffset + (size_t)(P.kv_head0_global + kvh) * HS, j, hp);
             char *krow = (char *)row_ptr(pos);
             knew[j] = kv_q8_append(krow, P.kv.kv_len, xoff + blk * 32, r);
-            vnew[j] = kv_q8_append(krow + v_off, P.kv.kv_len, xoff + blk * 32, __ldcg(P.v + (size_t)m * P.kv_seg + xoff + j));
+            vnew[j] = kv_q8_append(krow + v_off, P.kv.kv_len, xoff + blk * 32, __ldcg(P.v + (size_t)m * P.kv_ld + xoff + j));
         }
     } else if (owner) {
         for (int j = NT - 1 - tid; j < hp; j += NT) { // the warps the q loop leaves idle
             const float2 f = __ldg((const float2 *)P.rope + poffset + (size_t)(P.kv_head0_global + kvh) * HS + j);
-            const float *kr = P.k + (size_t)m * P.kv_seg + xoff, *vr = P.v + (size_t)m * P.kv_seg + xoff;
+            const float *kr = P.k + (size_t)m * P.kv_ld + xoff, *vr = P.v + (size_t)m * P.kv_ld + xoff;
             const float k0 = __ldcg(kr + j), k1 = __ldcg(kr + j + hp);
             const float v0 = __ldcg(vr + j), v1 = __ldcg(vr + j + hp);
             const float r0 = __fsub_rn(__fmul_rn(k0, f.x), __fmul_rn(k1, f.y));
@@ -141,7 +140,7 @@ __device__ __forceinline__ void attention_flat(const AttnTask &P, const int laye
                 ((float *)vrow)[xoff + j] = v0, ((float *)vrow)[xoff + j + hp] = v1;
                 knew[j] = r0, knew[j + hp] = r1, vnew[j] = v0, vnew[j + hp] = v1;
             } else { // the scores see the values as stored (bf16-rounded), like a later read of the page would
-                const uint16_t b0 = mg_bf16(r0), b1 = mg_bf16(r1), c0 = mg_bf16(v0), c1 = mg_bf16(v1);
+                const uint16_t b0 = f32_to_bf16_rne(r0), b1 = f32_to_bf16_rne(r1), c0 = f32_to_bf16_rne(v0), c1 = f32_to_bf16_rne(v1);
                 ((uint16_t *)krow)[xoff + j] = b0, ((uint16_t *)krow)[xoff + j + hp] = b1;
                 ((uint16_t *)vrow)[xoff + j] = c0, ((uint16_t *)vrow)[xoff + j + hp] = c1;
                 knew[j] = bf16_bits_to_f32(b0), knew[j + hp] = bf16_bits_to_f32(b1);
@@ -175,7 +174,7 @@ __device__ __forceinline__ void attention_flat(const AttnTask &P, const int laye
             a += __shfl_xor_sync(0xffffffffu, a, 1);
             a += __shfl_xor_sync(0xffffffffu, a, 2);
             a += __shfl_xor_sync(0xffffffffu, a, 4);
-            if (sg == 0 && position < t1) S[pl * group + h] = __fmul_rn(a, P.attn_scale);
+            if (sg == 0 && position < t1) S[pl * group + h] = __fmul_rn(a, P.scale);
         }
     }
     task_bar<NT>(); // (2) scores complete
@@ -261,9 +260,9 @@ __device__ __forceinline__ void attention_flat(const AttnTask &P, const int laye
 #pragma unroll
             for (int w = 0; w < NW; w++) L += wsum[w * MG_MAX_GROUP + hb + h];
             if (Sp == 1) {
-                P.att[(size_t)m * P.attn_seg + (h0 + hb + h) * HS + d] = cnt > 0 ? __fdiv_rn(a, L) : 0.0f;
+                P.out[(size_t)m * P.q_ld + (h0 + hb + h) * HS + d] = cnt > 0 ? __fdiv_rn(a, L) : 0.0f;
             } else {
-                float *wsp = P.attn_ws + (((size_t)m * P.heads + h0 + hb + h) * Sp + split) * (HS + 2);
+                float *wsp = P.ws + (((size_t)m * P.heads + h0 + hb + h) * Sp + split) * (HS + 2);
                 wsp[d] = a;
                 if (d == 0) {
                     float Mh = -INFINITY;

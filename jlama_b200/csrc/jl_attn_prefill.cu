@@ -288,13 +288,10 @@ static int launch_pa(jl_ctx *ctx, cudaStream_t s, const AttnParams &p, int sessi
 template <bool TAB>
 static int launch_pa_any(jl_ctx *ctx, cudaStream_t s, const AttnParams &p, int session, int pos0, const int4 *tab, int ntab) {
     if (!jl_prefill_attention_supported(p)) return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "prefill attention: unsupported head shape");
-    if (p.kv.kv_dtype == JL_I8)
-        return p.head_size == 64 ? launch_pa<64, JL_I8, TAB>(ctx, s, p, session, pos0, tab, ntab) : launch_pa<128, JL_I8, TAB>(ctx, s, p, session, pos0, tab, ntab);
-    if (p.head_size == 64)
-        return p.kv.kv_dtype == JL_F32 ? launch_pa<64, JL_F32, TAB>(ctx, s, p, session, pos0, tab, ntab)
-                                       : launch_pa<64, JL_BF16, TAB>(ctx, s, p, session, pos0, tab, ntab);
-    return p.kv.kv_dtype == JL_F32 ? launch_pa<128, JL_F32, TAB>(ctx, s, p, session, pos0, tab, ntab)
-                                   : launch_pa<128, JL_BF16, TAB>(ctx, s, p, session, pos0, tab, ntab);
+    return kv_dispatch<true>(p.kv.kv_dtype, [&](auto t) {
+        constexpr int KVDT = decltype(t)::value;
+        return p.head_size == 64 ? launch_pa<64, KVDT, TAB>(ctx, s, p, session, pos0, tab, ntab) : launch_pa<128, KVDT, TAB>(ctx, s, p, session, pos0, tab, ntab);
+    });
 }
 
 // rows p.rows of one session at positions pos0 .. pos0 + rows - 1; q is post-RoPE, the chunk's own K/V are already in the pages

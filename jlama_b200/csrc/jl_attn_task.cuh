@@ -1,22 +1,11 @@
-// Shared device code of the decode attention task: one (row, kv head, context split) per CTA-sized thread group.
-// Used by the persistent megakernel (jl_mega.cu, NT = its consumer threads) and by the stand-alone fused decode
-// attention kernel (jl_attention.cu).  CausalSelfAttention.java:199-356.
+// Shared device code of the decode attention tasks: one (row, kv head, context split) per CTA-sized thread group.
+// The tiled task is run by the stand-alone fused decode attention kernel (jl_attention.cu); the flat task (jl_attn_flat.cuh) and
+// attention_merge also by the persistent decode kernel (jl_pdecode.cu, NT = its threads).  CausalSelfAttention.java:199-356.
 #pragma once
 #include "jl_common.cuh"
 
 #define MG_ATT_TILE 32
 #define MG_MAX_GROUP 8
-
-struct AttnTask {
-    int heads, kv_heads, head_size, attn_seg, kv_seg, kv_head0_global, splits;
-    float attn_scale;
-    const float *q, *k, *v; // raw projections of this step [rows, attn_seg] / [rows, kv_seg]
-    float *att;             // [rows, attn_seg]
-    float *attn_ws;         // [rows, heads, splits, hs + 2] split partials
-    const float *rope;
-    KvLayout kv;
-    const int32_t *sessions, *positions;
-};
 
 // softmax exponent exactly as the reference computes it: (float)Math.exp((double)x) (one out-of-line copy: the double exp
 // is ~150 instructions and the attention kernel starts with a cold instruction cache every layer)
@@ -40,23 +29,6 @@ __host__ __device__ constexpr size_t attention_task_smem() {
            (size_t)2 * HS * 4 + (size_t)(NT / HS) * MG_MAX_GROUP * HS * 4;
 }
 
-__device__ __forceinline__ const char *mg_kv_row(const KvLayout &kv, int session, int layer, int pos, int which) {
-    const int lp = layer / kv.layers_per_page, rl = layer % kv.layers_per_page;
-    const int cp = pos / kv.ctx_per_page, rc = pos % kv.ctx_per_page;
-    const char *base = (const char *)kv.page_table[((size_t)session * kv.n_layer_pages + lp) * kv.n_ctx_pages + cp];
-    return base + (((size_t)rl * 2 + which) * kv.ctx_per_page + rc) * kv_row_bytes(kv.kv_dtype, kv.kv_len);
-}
-__device__ __forceinline__ uint16_t mg_bf16(float n) {
-    const uint32_t nbits = __float_as_uint(n);
-    const uint32_t s = (nbits >> 16) & 0x8000u, e = (nbits >> 16) & 0x7f80u, m = nbits & 0x7fffffu;
-    if (e != 0x7f80u) {
-        const int mshift = (int)(m >> 16), masked = (int)(m & 0xffff), cmp = masked - 0x8000;
-        const int m1 = cmp > 0 ? mshift + 1 : (cmp < 0 ? mshift : ((mshift & 1) ? mshift + 1 : mshift));
-        return (uint16_t)(s | (e + (uint32_t)m1));
-    }
-    return m != 0 ? (uint16_t)0x7fc0 : (uint16_t)(nbits >> 16);
-}
-
 // One (row m, kv head, split) task.  smem `u` (sized by uarea_bytes) aliases the
 // activation staging area, which is dead between the QKV stages and the o_proj prologue.
 // Latency plan: the RoPE inputs, the KV append and the first K/V tile are all requested before the first
@@ -65,7 +37,7 @@ __device__ __forceinline__ uint16_t mg_bf16(float n) {
 // KVDT: JL_F32 / JL_BF16 / JL_I8 fix the page element type at compile time (half the fetch / append code); -1 = F32 or BF16 at run
 // time.  I8 rows are prefetched raw and dequantised as the tile is staged; the owner's append quantises one 32-element block per warp.
 template <int HS, int NT, int KVDT = -1>
-__device__ void attention_task(const AttnTask &P, int layer, int m, int kvh, int split, unsigned char *u) {
+__device__ void attention_task(const AttnParams &P, int m, int kvh, int split, unsigned char *u) {
     constexpr int C4 = HS / 4;
     constexpr int PARTS = NT / HS; // P.V position groups
     constexpr int NF = (MG_ATT_TILE * C4 + NT - 1) / NT; // float4 per thread per tile
@@ -94,7 +66,7 @@ __device__ void attention_task(const AttnTask &P, int layer, int m, int kvh, int
 
     // page addressing (KvBufferCache.java:160-199 geometry): the layer split is fixed for the task, the context split is
     // resolved once per tile (a tile of consecutive positions touches at most two pages when ctx_per_page >= TILE)
-    const int lpage = layer / P.kv.layers_per_page, rlayer = layer - lpage * P.kv.layers_per_page;
+    const int lpage = P.layer / P.kv.layers_per_page, rlayer = P.layer - lpage * P.kv.layers_per_page;
     const size_t v_off = kv_rows_bytes<KVDT>(dt, P.kv.kv_len, P.kv.ctx_per_page); // K block -> V block of the same layer
     const size_t layer_off = kv_rows_bytes<KVDT>(dt, P.kv.kv_len, (size_t)rlayer * 2 * P.kv.ctx_per_page);
     char *const *ptab = (char *const *)P.kv.page_table + ((size_t)session * P.kv.n_layer_pages + lpage) * P.kv.n_ctx_pages;
@@ -141,7 +113,7 @@ __device__ void attention_task(const AttnTask &P, int layer, int m, int kvh, int
     for (int idx = tid; idx < group * hp; idx += NT) {
         const int h = idx / hp, j = idx % hp;
         const float2 f = __ldg((const float2 *)P.rope + poffset + (size_t)(P.kv_head0_global + kvh) * HS + j);
-        const float *qr = P.q + (size_t)m * P.attn_seg + (h0 + h) * HS;
+        const float *qr = P.q + (size_t)m * P.q_ld + (h0 + h) * HS;
         const float q0 = __ldcg(qr + j), q1 = __ldcg(qr + j + hp);
         qs[h * HS + j] = __fsub_rn(__fmul_rn(q0, f.x), __fmul_rn(q1, f.y));
         qs[h * HS + j + hp] = __fadd_rn(__fmul_rn(q0, f.y), __fmul_rn(q1, f.x));
@@ -153,15 +125,15 @@ __device__ void attention_task(const AttnTask &P, int layer, int m, int kvh, int
         const int blk = NT / 32 - 1 - warp;
         if (owner && blk < HS / 32) {
             const int j = blk * 32 + lane;
-            const float r = rope_key_elem(P.k + (size_t)m * P.kv_seg + xoff, (const float2 *)P.rope + poffset + (size_t)(P.kv_head0_global + kvh) * HS, j, hp);
+            const float r = rope_key_elem(P.k + (size_t)m * P.kv_ld + xoff, (const float2 *)P.rope + poffset + (size_t)(P.kv_head0_global + kvh) * HS, j, hp);
             char *krow = k_row(pos);
             knew[j] = kv_q8_append(krow, P.kv.kv_len, xoff + blk * 32, r);
-            vnew[j] = kv_q8_append(krow + v_off, P.kv.kv_len, xoff + blk * 32, __ldcg(P.v + (size_t)m * P.kv_seg + xoff + j));
+            vnew[j] = kv_q8_append(krow + v_off, P.kv.kv_len, xoff + blk * 32, __ldcg(P.v + (size_t)m * P.kv_ld + xoff + j));
         }
     } else if (owner) {
         for (int j = NT - 1 - tid; j < hp; j += NT) { // use the warps the q loop leaves idle
             const float2 f = __ldg((const float2 *)P.rope + poffset + (size_t)(P.kv_head0_global + kvh) * HS + j);
-            const float *kr = P.k + (size_t)m * P.kv_seg + xoff, *vr = P.v + (size_t)m * P.kv_seg + xoff;
+            const float *kr = P.k + (size_t)m * P.kv_ld + xoff, *vr = P.v + (size_t)m * P.kv_ld + xoff;
             const float k0 = __ldcg(kr + j), k1 = __ldcg(kr + j + hp);
             const float v0 = __ldcg(vr + j), v1 = __ldcg(vr + j + hp);
             float r0 = __fsub_rn(__fmul_rn(k0, f.x), __fmul_rn(k1, f.y));
@@ -173,7 +145,7 @@ __device__ void attention_task(const AttnTask &P, int layer, int m, int kvh, int
                 ((float *)vrow)[xoff + j] = v0, ((float *)vrow)[xoff + j + hp] = v1;
                 knew[j] = r0, knew[j + hp] = r1, vnew[j] = v0, vnew[j + hp] = v1;
             } else { // the scores see the values as stored (bf16-rounded), like a later read of the page would
-                const uint16_t b0 = mg_bf16(r0), b1 = mg_bf16(r1), c0 = mg_bf16(v0), c1 = mg_bf16(v1);
+                const uint16_t b0 = f32_to_bf16_rne(r0), b1 = f32_to_bf16_rne(r1), c0 = f32_to_bf16_rne(v0), c1 = f32_to_bf16_rne(v1);
                 ((uint16_t *)krow)[xoff + j] = b0, ((uint16_t *)krow)[xoff + j + hp] = b1;
                 ((uint16_t *)vrow)[xoff + j] = c0, ((uint16_t *)vrow)[xoff + j + hp] = c1;
                 knew[j] = bf16_bits_to_f32(b0), knew[j + hp] = bf16_bits_to_f32(b1);
@@ -230,7 +202,7 @@ __device__ void attention_task(const AttnTask &P, int layer, int m, int kvh, int
             }
             a += __shfl_xor_sync(0xffffffffu, a, 1);
             a += __shfl_xor_sync(0xffffffffu, a, 2);
-            if (qd == 0) ps[t * MG_MAX_GROUP + h] = t < cnt ? __fmul_rn(a, P.attn_scale) : -INFINITY;
+            if (qd == 0) ps[t * MG_MAX_GROUP + h] = t < cnt ? __fmul_rn(a, P.scale) : -INFINITY;
         }
         task_bar<NT>();
         // online softmax: warp h owns head h (TILE == 32: one score per lane)
@@ -271,9 +243,9 @@ __device__ void attention_task(const AttnTask &P, int layer, int m, int kvh, int
             float a = 0.0f;
             for (int pp = 0; pp < PARTS; pp++) a += comb[((size_t)pp * MG_MAX_GROUP + h) * HS + d];
             if (S == 1) {
-                P.att[(size_t)m * P.attn_seg + (h0 + h) * HS + d] = t0 < t1 ? __fdiv_rn(a, hl[h]) : 0.0f;
+                P.out[(size_t)m * P.q_ld + (h0 + h) * HS + d] = t0 < t1 ? __fdiv_rn(a, hl[h]) : 0.0f;
             } else {
-                float *w = P.attn_ws + (((size_t)m * P.heads + h0 + h) * S + split) * (HS + 2);
+                float *w = P.ws + (((size_t)m * P.heads + h0 + h) * S + split) * (HS + 2);
                 w[d] = a;
                 if (d == 0) w[HS] = hm[h], w[HS + 1] = hl[h];
             }
@@ -283,14 +255,14 @@ __device__ void attention_task(const AttnTask &P, int layer, int m, int kvh, int
 
 // merge the split partials of one (row, kv head): out = sum_s acc_s*exp(m_s-M) / sum_s l_s*exp(m_s-M)
 template <int HS, int NT>
-__device__ void attention_merge(const AttnTask &P, int m, int kvh, unsigned char *u) {
+__device__ void attention_merge(const AttnParams &P, int m, int kvh, unsigned char *u) {
     const int group = P.heads / P.kv_heads, S = P.splits;
     // rescaling factors exp(m_s - M), one per (head, split), computed once (one exponential deep) instead of S serial
     // exponentials in every (head, d) thread
     float *fac = (float *)u; // [group][S] in the task's shared-memory area (dead once the task's partials are written)
     for (int idx = threadIdx.x; idx < group * S; idx += NT) {
         const int hl = idx / S, s = idx - hl * S;
-        const float *w = P.attn_ws + ((size_t)m * P.heads + kvh * group + hl) * S * (HS + 2);
+        const float *w = P.ws + ((size_t)m * P.heads + kvh * group + hl) * S * (HS + 2);
         float M = -INFINITY;
         for (int t = 0; t < S; t++) M = fmaxf(M, __ldcg(w + t * (HS + 2) + HS));
         const float ms = __ldcg(w + s * (HS + 2) + HS);
@@ -299,7 +271,7 @@ __device__ void attention_merge(const AttnTask &P, int m, int kvh, unsigned char
     task_bar<NT>(); // all NT task threads call this function (whole CTA in the fused kernel, the consumer warps in the megakernel)
     for (int idx = threadIdx.x; idx < group * HS; idx += NT) {
         const int hl = idx / HS, h = kvh * group + hl, d = idx % HS;
-        const float *w = P.attn_ws + ((size_t)m * P.heads + h) * S * (HS + 2);
+        const float *w = P.ws + ((size_t)m * P.heads + h) * S * (HS + 2);
         float num = 0.0f, den = 0.0f;
         for (int s = 0; s < S; s++) {
             const float f = fac[hl * S + s];
@@ -307,6 +279,6 @@ __device__ void attention_merge(const AttnTask &P, int m, int kvh, unsigned char
             num = fmaf(__ldcg(w + s * (HS + 2) + d), f, num);
             den = fmaf(__ldcg(w + s * (HS + 2) + HS + 1), f, den);
         }
-        P.att[(size_t)m * P.attn_seg + h * HS + d] = __fdiv_rn(num, den);
+        P.out[(size_t)m * P.q_ld + h * HS + d] = __fdiv_rn(num, den);
     }
 }

@@ -6,6 +6,7 @@
 #include <stdint.h>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 
@@ -280,9 +281,10 @@ struct KvLayout {
 // value i of the block reads as __fmul_rn((float)q, scale).  head_size is a multiple of 32, so KV head h owns whole blocks: its int8
 // values start at byte h * head_size and its scales at kv_q8_scale_off(kv_len, h * head_size).
 // kv_rows_bytes: the bytes of `rows` consecutive rows, i.e. the offset of row `rows` of a page.  KVDT: the dtype when a kernel fixes
-// it at compile time; -1 = `dt` at run time, F32 or BF16 only: a -1 instantiation addresses I8 pages as 2 bytes per element.  The
-// launchers send I8 layouts to JL_I8 instantiations only, and the persistent decode kernel (attention_flat<HS, PD_NT>, -1) is kept off
-// I8 models by pd_ok in jl_model_finalize.
+// it at compile time; -1 = `dt` at run time, F32 or BF16 only: a -1 instantiation addresses I8 pages as 2 bytes per element.  So a
+// host launcher picks KVDT with kv_dispatch, which sends I8 layouts to JL_I8 instantiations only; the persistent decode kernel
+// (attention_flat<HS, PD_NT>, -1) is kept off I8 models by pd_ok in jl_model_finalize.  F32 / BF16 offsets keep the element-count
+// form rows * kv_len * bytes, which is what their instantiations are register-allocated with (DESIGN §3.16).
 template <int KVDT = -1>
 __host__ __device__ __forceinline__ size_t kv_rows_bytes(int dt, size_t kv_len, size_t rows) {
     if constexpr (KVDT == JL_I8) return rows * (kv_len + kv_len / 8);
@@ -298,6 +300,19 @@ __host__ __device__ __forceinline__ size_t kv_q8_scale_off(size_t kv_len, size_t
 __device__ __forceinline__ float4 kv_q8x4(uint32_t w, float s) {
     return make_float4(__fmul_rn((float)((int)(w << 24) >> 24), s), __fmul_rn((float)((int)(w << 16) >> 24), s),
                        __fmul_rn((float)((int)(w << 8) >> 24), s), __fmul_rn((float)((int)w >> 24), s));
+}
+
+// f(std::integral_constant<int, KVDT>) with the instantiation that reads pages of dtype dt: JL_I8 for I8 pages.  F32 and BF16 pages
+// get their own JL_F32 / JL_BF16 instantiations where the kernel has them (CONCRETE), and share the run-time -1 one otherwise.
+template <bool CONCRETE, typename F>
+static inline auto kv_dispatch(int dt, F &&f) -> decltype(f(std::integral_constant<int, JL_I8>())) {
+    if (dt == JL_I8) return f(std::integral_constant<int, JL_I8>());
+    if constexpr (CONCRETE) {
+        if (dt == JL_F32) return f(std::integral_constant<int, JL_F32>());
+        return f(std::integral_constant<int, JL_BF16>());
+    } else {
+        return f(std::integral_constant<int, -1>());
+    }
 }
 
 struct AttnParams {
@@ -324,7 +339,7 @@ struct AttnParams {
 // Writes rotated K and V of every row into the pages and rotates q in place (CausalSelfAttention.java:199-311).
 int jl_launch_rope_kv_append(jl_ctx *ctx, cudaStream_t s, const AttnParams &p, float *q_inplace);
 // Causal attention of each row against positions [0, pos] of its session (CausalSelfAttention.java:314-356).
-int jl_launch_paged_attention(jl_ctx *ctx, cudaStream_t s, const AttnParams &p, int max_pos);
+int jl_launch_paged_attention(jl_ctx *ctx, cudaStream_t s, const AttnParams &p);
 // tiled prefill attention for one session's chunk of consecutive positions (jl_attn_prefill.cu)
 bool jl_prefill_attention_supported(const AttnParams &p);
 int jl_launch_prefill_attention(jl_ctx *ctx, cudaStream_t s, const AttnParams &p, int session, int pos0);
@@ -440,6 +455,17 @@ inline unsigned long long *jl_ktrace_slot(jl_ctx *ctx) {
 }
 
 __device__ __forceinline__ float bf16_bits_to_f32(uint16_t b) { return __uint_as_float(((uint32_t)b) << 16); }
+// f32 -> bf16 round to nearest even, NaN preserving (FloatConversions.java:35-61)
+__device__ __forceinline__ uint16_t f32_to_bf16_rne(float n) {
+    const uint32_t nbits = __float_as_uint(n);
+    const uint32_t s = (nbits >> 16) & 0x8000u, e = (nbits >> 16) & 0x7f80u, m = nbits & 0x7fffffu;
+    if (e != 0x7f80u) {
+        const int mshift = (int)(m >> 16), masked = (int)(m & 0xffff), cmp = masked - 0x8000;
+        const int m1 = cmp > 0 ? mshift + 1 : (cmp < 0 ? mshift : ((mshift & 1) ? mshift + 1 : mshift));
+        return (uint16_t)(s | (e + (uint32_t)m1));
+    }
+    return m != 0 ? (uint16_t)0x7fc0 : (uint16_t)(nbits >> 16);
+}
 
 // Q8_0 block quantiser (Q8ByteBufferTensor.java:47-90), warp-collective: lane l holds element l of one 32-element block and gets its
 // int8 value back; *scale = the block's scale.  max from Float.MIN_VALUE, iscale = 127 / max, q = (byte)Math.round(x * iscale),

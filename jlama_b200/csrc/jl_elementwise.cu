@@ -115,21 +115,11 @@ int jl_launch_quantize_q8(jl_ctx *ctx, cudaStream_t s, const float *x, int rows,
     return JL_OK;
 }
 
-// ---- f32 -> bf16 RNE, NaN preserving (FloatConversions.java:35-61) -------------------------------------------
-__device__ __forceinline__ uint16_t f32_to_bf16_ref(float n) {
-    const uint32_t nbits = __float_as_uint(n);
-    const uint32_t s = (nbits >> 16) & 0x8000u, e = (nbits >> 16) & 0x7f80u, m = nbits & 0x7fffffu;
-    if (e != 0x7f80u) {
-        const int mshift = (int)(m >> 16), masked = (int)(m & 0xffff), cmp = masked - 0x8000;
-        const int m1 = cmp > 0 ? mshift + 1 : (cmp < 0 ? mshift : ((mshift & 1) ? mshift + 1 : mshift));
-        return (uint16_t)(s | (e + (uint32_t)m1));
-    }
-    return m != 0 ? (uint16_t)0x7fc0 : (uint16_t)(nbits >> 16);
-}
+// ---- f32 -> bf16 RNE, NaN preserving (f32_to_bf16_rne, FloatConversions.java:35-61) ---------------------------------
 __global__ void quantize_bf16_kernel(const float *x, int ldx, int offset, int length, uint16_t *out) {
     const int r = blockIdx.y;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < length; i += gridDim.x * blockDim.x)
-        out[(size_t)r * ldx + offset + i] = f32_to_bf16_ref(x[(size_t)r * ldx + offset + i]);
+        out[(size_t)r * ldx + offset + i] = f32_to_bf16_rne(x[(size_t)r * ldx + offset + i]);
 }
 int jl_launch_quantize_bf16(jl_ctx *ctx, cudaStream_t s, const float *x, int rows, int ldx, int offset, int length,
                             uint16_t *out) {
@@ -167,7 +157,7 @@ __global__ void rmsnorm_bf16_kernel(const float *x, int ldx, int w_dtype, const 
     const float rsf = rs_sh;
     for (int i = tid; i < E; i += blockDim.x) {
         const float wv = w_dtype == JL_BF16 ? bf16_bits_to_f32(((const uint16_t *)w)[i]) : ((const float *)w)[i];
-        out[(size_t)r * ldo + i] = f32_to_bf16_ref(__fmul_rn(__fadd_rn(adj, wv), __fmul_rn(rsf, xr[i])));
+        out[(size_t)r * ldo + i] = f32_to_bf16_rne(__fmul_rn(__fadd_rn(adj, wv), __fmul_rn(rsf, xr[i])));
     }
 }
 int jl_launch_rmsnorm_bf16(jl_ctx *ctx, cudaStream_t s, const float *x, int rows, int ldx, int w_dtype, const void *w, float adj, float eps,
@@ -190,8 +180,8 @@ __global__ void silu_mul_bf16_kernel(const float *gate, const float *up, int ld,
         const float w[4] = {u.x, u.y, u.z, u.w};
 #pragma unroll
         for (int k = 0; k < 4; k++) v[k] = __fmul_rn(__fdividef(v[k], 1.0f + __expf(-v[k])), w[k]);
-        o2[i] = make_uint2((uint32_t)f32_to_bf16_ref(v[0]) | ((uint32_t)f32_to_bf16_ref(v[1]) << 16),
-                           (uint32_t)f32_to_bf16_ref(v[2]) | ((uint32_t)f32_to_bf16_ref(v[3]) << 16));
+        o2[i] = make_uint2((uint32_t)f32_to_bf16_rne(v[0]) | ((uint32_t)f32_to_bf16_rne(v[1]) << 16),
+                           (uint32_t)f32_to_bf16_rne(v[2]) | ((uint32_t)f32_to_bf16_rne(v[3]) << 16));
     }
 }
 int jl_launch_silu_mul_bf16(jl_ctx *ctx, cudaStream_t s, const float *gate, const float *up, int rows, int ld, int length, uint16_t *out, int ldo) {

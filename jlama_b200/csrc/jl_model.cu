@@ -895,21 +895,21 @@ static AttnParams attn_params(const jl_model *m, int L, int M, int splits) {
 // decode (one row per session): one fused kernel, `splits` = about one per 64 positions.  The launch may be replayed from a graph
 // for every context of its split bucket (run_decode), so the kernel is chosen by the largest position the bucket can see, not by
 // the current one.
-static int attention(jl_model *m, int L, int M, int max_pos, int splits, bool decode) {
+static int attention(jl_model *m, int L, int M, int splits, bool decode) {
     const AttnParams ap = attn_params(m, L, M, splits);
     if (decode) {
         const int bound = splits >= m->max_splits ? m->max_context - 1 : splits * 64 * M - 1;
         return jl_launch_fused_decode_attention(m->ctx, m->stream, ap, m->fda_done, bound);
     }
     M_CHECK(jl_launch_rope_kv_append(m->ctx, m->stream, ap, m->q));
-    return jl_launch_paged_attention(m->ctx, m->stream, ap, max_pos);
+    return jl_launch_paged_attention(m->ctx, m->stream, ap);
 }
 
 // AbstractModel.forward (:314-329) over M rows whose tokens/positions/sessions are already on the device.
-static int forward_rows_gpt2(jl_model *m, int M, int max_pos, int splits, bool distinct_sessions);
+static int forward_rows_gpt2(jl_model *m, int M, int splits, bool distinct_sessions);
 
-static int forward_rows(jl_model *m, int M, int max_pos, int splits, bool distinct_sessions = false) {
-    if (m->cfg.arch == JL_ARCH_GPT2) return forward_rows_gpt2(m, M, max_pos, splits, distinct_sessions);
+static int forward_rows(jl_model *m, int M, int splits, bool distinct_sessions = false) {
+    if (m->cfg.arch == JL_ARCH_GPT2) return forward_rows_gpt2(m, M, splits, distinct_sessions);
     jl_ctx *ctx = m->ctx;
     const jl_model_config &c = m->cfg;
     const int E = c.embedding_length;
@@ -929,7 +929,7 @@ static int forward_rows(jl_model *m, int M, int max_pos, int splits, bool distin
             set_norm(p, lw[JL_L_ATTN_NORM], m);
             M_CHECK(run_gemm(m, p, act_q(lw[JL_L_Q]) ? PRO_RMSNORM_QUANT : PRO_RMSNORM_F32, EPI_STORE, M, distinct_sessions));
         }
-        M_CHECK(attention(m, L, M, max_pos, splits, distinct_sessions));
+        M_CHECK(attention(m, L, M, splits, distinct_sessions));
         // ---- o_proj (+ reducer) + residual (CausalSelfAttention.java:363-378, TransformerBlock.java:185) ----
         {
             const bool tp = c.tp_size > 1;
@@ -1035,7 +1035,7 @@ static int stage_rows(jl_model *m, int n, const int32_t *tokens, const int32_t *
 // (BF16 operands, F32 accumulate; jl_gemm_tc.cu).  Norms, RoPE, attention, SiLU stay f32.
 // segs[i] = {session, pos0, first row, rows} (HOST): the M rows are nseg runs of consecutive positions, one per session.  Every op but
 // the attention works row by row; one segment takes the single-session tiled attention, several take its block-table variant.
-static int forward_rows_tc(jl_model *m, int M, int max_pos, int splits, const int4 *segs, int nseg) {
+static int forward_rows_tc(jl_model *m, int M, int splits, const int4 *segs, int nseg) {
     jl_ctx *ctx = m->ctx;
     const jl_model_config &c = m->cfg;
     const int E = c.embedding_length, H = m->h_seg;
@@ -1052,7 +1052,7 @@ static int forward_rows_tc(jl_model *m, int M, int max_pos, int splits, const in
         M_CHECK(jl_launch_rope_kv_append(ctx, m->stream, ap, m->q));
         // rows = consecutive positions pos0.. of one session per segment: tiled tensor-core attention (jl_attn_prefill.cu)
         if (!jl_prefill_attention_supported(ap)) {
-            M_CHECK(jl_launch_paged_attention(ctx, m->stream, ap, max_pos));
+            M_CHECK(jl_launch_paged_attention(ctx, m->stream, ap));
         } else if (nseg == 1) {
             M_CHECK(jl_launch_prefill_attention(ctx, m->stream, ap, segs[0].x, segs[0].y));
         } else {
@@ -1079,7 +1079,7 @@ static int forward_rows_tc(jl_model *m, int M, int max_pos, int splits, const in
 //   ln2 = LayerNorm(xb) -> h = gelu(ln2 . Wfc^T + bfc) -> x = (h . Wproj^T + bproj) + xb
 // in the order TransformerBlock.forward / CausalSelfAttention.forward / MLPBlock.forward apply them (bias after the reducer,
 // residual last: CausalSelfAttention.java:363-380, MLPBlock.java:126-160, TransformerBlock.java:185,203).
-static int forward_rows_gpt2(jl_model *m, int M, int max_pos, int splits, bool distinct_sessions) {
+static int forward_rows_gpt2(jl_model *m, int M, int splits, bool distinct_sessions) {
     jl_ctx *ctx = m->ctx;
     const jl_model_config &c = m->cfg;
     const int E = c.embedding_length, H = m->h_seg;
@@ -1109,7 +1109,7 @@ static int forward_rows_gpt2(jl_model *m, int M, int max_pos, int splits, bool d
         M_CHECK(bias(m->q, m->attn_seg, ax[JL_AUX_Q_BIAS], m->attn_seg));
         M_CHECK(bias(m->k, m->kv_seg, ax[JL_AUX_K_BIAS], m->kv_seg));
         M_CHECK(bias(m->v, m->kv_seg, ax[JL_AUX_V_BIAS], m->kv_seg));
-        M_CHECK(attention(m, L, M, max_pos, splits, distinct_sessions));
+        M_CHECK(attention(m, L, M, splits, distinct_sessions));
         M_CHECK(gemm(gemv_params(lw[JL_L_O], m->xb, E, m->att, m->attn_seg, E), lw[JL_L_O]));
         M_CHECK(bias(m->xb, E, ax[JL_AUX_O_BIAS], E));
         M_CHECK(jl_launch_accumulate(ctx, m->stream, m->xb, M, E, JL_F32, m->x, nullptr, M, E, 0, E)); // + residual
@@ -1275,8 +1275,8 @@ static int forward_chunks(jl_model *m, const std::vector<PrefillChunk> &ch, bool
     M_CHECK(stage_rows(m, M, tokens.data(), positions.data(), sessions.data()));
     JL_CUDA_CHECK(ctx, cudaMemcpyAsync(m->d_rows, rows, (size_t)(S + n) * 4, cudaMemcpyHostToDevice, m->stream));
     const int splits = pick_splits(m, max_pos, M);
-    if (tc) M_CHECK(forward_rows_tc(m, M, max_pos, splits, segs.data(), n));
-    else M_CHECK(forward_rows(m, M, max_pos, splits));
+    if (tc) M_CHECK(forward_rows_tc(m, M, splits, segs.data(), n));
+    else M_CHECK(forward_rows(m, M, splits));
     if (so) M_CHECK(score_pass(m, ch, so->top_n));
     M_CHECK(copy_rows(m, m->last_hidden, m->d_rows + S, m->x, m->d_rows, n));
     JL_CUDA_CHECK(ctx, cudaStreamSynchronize(m->stream)); // pinned staging is reused by the next pass
@@ -1440,9 +1440,9 @@ __global__ void advance_kernel(int32_t *tokens, int32_t *positions, const int32_
     if (i == 0) *counter = cnt + 1;
 }
 
-static int decode_body(jl_model *m, int n, int max_pos, int splits, bool resident) {
+static int decode_body(jl_model *m, int n, int splits, bool resident) {
     jl_ctx *ctx = m->ctx;
-    M_CHECK(forward_rows(m, n, max_pos, splits, true));
+    M_CHECK(forward_rows(m, n, splits, true));
     M_CHECK(sample_rows(m, m->x, n));
     if (resident) {
         JL_CUDA_CHECK(ctx, jl_launch_kernel(advance_kernel, dim3(1), dim3(256), 0, m->stream, m->d_tokens, m->d_positions,
@@ -1529,7 +1529,7 @@ static int run_decode(jl_model *m, int n, int max_pos, bool resident, bool want_
             }
         splits = b > m->max_splits ? m->max_splits : b;
     }
-    if (!use_graph(m)) return decode_body(m, n, max_pos, splits, resident);
+    if (!use_graph(m)) return decode_body(m, n, splits, resident);
     const long long key = ((long long)n << 32) | ((long long)splits << 1) | (resident ? 1 : 0);
     auto it = m->graphs.find(key);
     if (it == m->graphs.end()) {
@@ -1544,7 +1544,7 @@ static int run_decode(jl_model *m, int n, int max_pos, bool resident, bool want_
             const long long before = ctx->launches;
             const int before_trace = ctx->ktrace_n;
             JL_CUDA_CHECK(ctx, cudaStreamBeginCapture(m->stream, cudaStreamCaptureModeThreadLocal));
-            int rc = decode_body(m, n, max_pos, sp, resident);
+            int rc = decode_body(m, n, sp, resident);
             cudaError_t ce = cudaStreamEndCapture(m->stream, &graph);
             const long long per_graph = ctx->launches - before;
             ctx->launches = before;

@@ -499,23 +499,17 @@ template <int HS>
 __device__ PD_PHASE_FN void pd_attention(const int, const int layer, const int kvh, const int split, const int splits, const bool merge,
                                          const unsigned long long qkv_target, unsigned char *smem) {
     PD_OPAQUE_ZERO(pz);
-    AttnTask at;
-    at.heads = CP.heads, at.kv_heads = CP.kv_heads, at.head_size = CP.head_size, at.attn_seg = CP.attn_seg, at.kv_seg = CP.kv_seg;
-    at.kv_head0_global = CP.kv_head0_global, at.splits = splits, at.attn_scale = CP.attn_scale;
-    at.q = CP.q, at.k = CP.k, at.v = CP.v, at.att = CP.att, at.attn_ws = CP.attn_ws, at.rope = CP.rope, at.kv = CP.kv;
-    at.sessions = CP.sessions, at.positions = CP.positions;
+    AttnParams at;
+    at.kv = CP.kv, at.layer = layer, at.heads = CP.heads, at.kv_heads = CP.kv_heads, at.head_size = CP.head_size;
+    at.kv_head0_global = CP.kv_head0_global, at.q = CP.q, at.k = CP.k, at.v = CP.v, at.q_ld = CP.attn_seg, at.kv_ld = CP.kv_seg;
+    at.out = CP.att, at.rope = CP.rope, at.sessions = CP.sessions, at.positions = CP.positions, at.scale = CP.attn_scale;
+    at.ws = CP.attn_ws, at.splits = splits, at.head0_global = 0, at.rows = 1; // (head0_global: only the per-op append reads it)
     if (merge) {
         attention_merge<HS, PD_NT>(at, 0, kvh, smem);
         return;
     }
-    const int group = at.heads / at.kv_heads;
-    const int n = at.positions[0] + 1;
-    const int per = (((n + splits - 1) / splits) + 31) / 32 * 32;
     // (the host only selects this kernel for power-of-two head groups and <= FA_MAX_POS positions per split)
-    (void)n;
-    (void)per;
-    (void)group;
-    attention_flat<HS, PD_NT>(at, layer, 0, kvh, split, smem, [&]() { pd_wait(pz, PC_QKV, qkv_target); });
+    attention_flat<HS, PD_NT>(at, 0, kvh, split, smem, [&]() { pd_wait(pz, PC_QKV, qkv_target); });
 }
 
 template <int WDT, int HS>
