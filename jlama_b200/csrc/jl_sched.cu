@@ -797,9 +797,20 @@ struct SlotJob { // what has to happen to a session slot before its new owner's 
     int64_t handle = -1;
     int attach = 0;
 };
+// how the token of one row of a sampling call is chosen
+struct Select {
+    float temperature = 0.0f, uniform = 0.0f;
+    int32_t top_k = 0;
+    float top_p = 1.0f;
+    bool filtered = false;
+    int32_t logprobs = -1;
+    const Penalty *pen = nullptr; // penalised request: its penalties, history = hist, whose first n_prompt tokens are its prompt
+    std::vector<int32_t> hist;
+    int n_prompt = 0;
+};
 struct PrefillJob {
     int64_t id;
-    int session, start, n, pos;
+    int session, n, pos;
     bool last;
     bool sibling = false;      // n-completion sibling: no prompt tokens; with `last` its first token is sampled after the leader's fork
     bool cancelled = false;    // leader cancelled before the fork: it forwards the prompt for its siblings but samples nothing
@@ -807,27 +818,11 @@ struct PrefillJob {
     uint64_t rng = 0;          // the request's uniform stream before the first-token draw, restored when the job is dropped
     std::vector<int32_t> retain; // prefix cache: the whole pages of a fresh prompt whose last chunk this job forwards
     std::vector<size_t> sibs;  // leader: the jobs of its siblings in this step
-    float temperature = 0.0f, uniform = 0.0f; // for the token sampled from the prompt's last row
-    int top_k = 0;
-    float top_p = 1.0f;
-    bool filtered = false;
-    int logprobs = -1;
-    const Penalty *pen = nullptr; // penalised request: its penalties, history = its prompt (hist)
-    std::vector<int32_t> hist;
+    Select sel;                // for the token sampled from the prompt's last row
     SlotJob slot;
     std::vector<int32_t> tokens;
-};
-struct Row {
-    int64_t id;
-    int32_t session, token, position;
-    float temperature, uniform;
-    int32_t top_k;
-    float top_p;
-    bool filtered;
-    int32_t logprobs;
-    const Penalty *pen = nullptr; // penalised request: its penalties, history = its prompt and generated tokens (hist, n_prompt)
-    std::vector<int32_t> hist;
-    int n_prompt = 0;
+    int rc = JL_OK;            // status of the job's backend calls
+    size_t call = 0, row = 0;  // its first token: row `row` of its group's first-token call `call`
 };
 
 // the jl_penalties of one backend call, row by row; rows without a Penalty are unpenalised with empty histories
@@ -849,18 +844,41 @@ struct PenCall {
     }
 };
 
-// the logprob outputs of one backend call, row by row
-struct LpOut {
+// the backend pair that serves a sampling call: the penalty pair when one of its rows is penalised, else the logprob pair when one wants
+// logprobs, else the top-k / top-p pair when one is filtered, else the plain calls
+enum Tier { PLAIN, TOPKP, LOGPROB, PENALTY };
+Tier tier_of(const Select &x) { return x.pen ? PENALTY : x.logprobs >= 0 ? LOGPROB : x.filtered ? TOPKP : PLAIN; }
+
+// the arguments and outputs of one sampling call (first tokens, or a decode step with its tokens and positions), row by row
+struct Call {
+    std::vector<int32_t> sessions, tokens, positions, top_k, top_n;
+    std::vector<float> temperatures, uniforms, top_p;
+    PenCall pc;
+    Tier tier = PLAIN;
+    std::vector<int32_t> next, top_ids; // the tokens; logprob and penalty calls also fill lp, top_ids and top_lp
     std::vector<float> lp, top_lp;
-    std::vector<int32_t> top_ids;
-    explicit LpOut(size_t n) : lp(n), top_lp(n * JL_MAX_LOGPROBS), top_ids(n * JL_MAX_LOGPROBS) {}
-    // row i -> the request's streams
-    void append_to(Request &r, size_t i) const {
+    explicit Call(size_t n) : next(n), top_ids(n * JL_MAX_LOGPROBS), lp(n), top_lp(n * JL_MAX_LOGPROBS) {}
+    void add(int32_t session, const Select &x) {
+        sessions.push_back(session), temperatures.push_back(x.temperature), uniforms.push_back(x.uniform);
+        top_k.push_back(x.top_k), top_p.push_back(x.top_p), top_n.push_back(x.logprobs);
+        pc.add(x.pen, x.hist, x.n_prompt);
+        tier = std::max(tier, tier_of(x));
+    }
+    // row i's logprobs -> the request's streams
+    void append_lp(Request &r, size_t i) const {
         const size_t W = JL_MAX_LOGPROBS;
         r.lp.push_back(lp[i]);
         r.top_ids.insert(r.top_ids.end(), top_ids.begin() + (long)(i * W), top_ids.begin() + (long)((i + 1) * W));
         r.top_lp.insert(r.top_lp.end(), top_lp.begin() + (long)(i * W), top_lp.begin() + (long)((i + 1) * W));
     }
+};
+
+// the work and outcome of one jl_sched_step
+struct Step {
+    jl_sched_stats st = {};
+    int first_error = JL_OK;
+    std::vector<PrefillJob> jobs;
+    std::vector<int64_t> discards; // spill handles of requests released since the last step
 };
 } // namespace
 
@@ -929,424 +947,403 @@ static int prepare_slot(jl_sched *s, PrefillJob &j, int *first_error) {
     return JL_OK;
 }
 
-extern "C" int jl_sched_step(jl_sched *s, jl_sched_stats *stats) {
-    if (!s) return JL_ERR_INVALID;
-    std::lock_guard<std::mutex> step_lock(s->step_mu);
-    jl_sched_stats st = {};
-    int first_error = JL_OK;
-    std::vector<PrefillJob> jobs;
-    std::unordered_map<int64_t, SlotJob> slot_jobs; // admitted this step: request id -> slot preparation
-    std::vector<int64_t> discards;
+// must hold s->mu.  Admit queued request `r`: into its parent's slot when the parent still holds its KV there (always possible), else, when
+// `may_take`, into a slot from take_slot, whose kept session is offloaded first.  False, with nothing changed, when it gets no slot.
+static bool admit(jl_sched *s, Request &r, bool may_take, std::unordered_map<int64_t, SlotJob> &slot_jobs, jl_sched_stats &st) {
+    SlotJob sj;
+    auto pa = r.parent >= 0 ? s->reqs.find(r.parent) : s->reqs.end();
+    if (pa != s->reqs.end() && pa->second.session >= 0) {
+        r.session = pa->second.session; // the parent's slot with its KV; ownership moves to the continuation
+        pa->second.session = -1;
+    } else {
+        int64_t victim = -1;
+        const int slot = may_take ? take_slot(s, &victim) : -1;
+        if (slot < 0) return false;
+        if (victim >= 0) {
+            Request &v = s->reqs[victim];
+            v.session = -1; // its KV leaves the device in this step (spill handle set when the offload returns)
+            v.spilling = true;
+            sj.victim = victim;
+            st.spilled++;
+        }
+        r.session = slot;
+        if (pa != s->reqs.end()) sj.restore_from = r.parent; // continuation of a spilled session
+        else sj.reset = true;
+    }
+    if (sj.reset && r.leader < 0 && s->prefix_max_pages > 0) {
+        // the longest cached whole-page prefix of the prompt that leaves its last token to forward, most recently used first (a
+        // sibling gets the leader's KV from the fork instead)
+        const int cpp = s->xb.ctx_per_page, pages = ((int)r.prompt.size() - 1) / cpp;
+        const std::vector<uint64_t> hashes = page_hashes(r.prompt.data(), pages, cpp);
+        s->pstats.lookups++;
+        for (int k = pages; k >= 1; k--) {
+            auto e = prefix_find(s, r.prompt.data(), k, hashes[(size_t)k - 1], false);
+            if (e == s->prefix.end()) continue;
+            e->second.last_use = s->step_no, e->second.pins++;
+            sj.reset = false, sj.entry = e->first, sj.handle = e->second.handle, sj.attach = k * cpp;
+            r.prefilled = r.cached = k * cpp;
+            break;
+        }
+    }
+    s->slot_owner[(size_t)r.session] = r.id;
+    r.state = JL_SCHED_PREFILL;
+    r.t_admit = r.leader >= 0 ? s->reqs[r.leader].t_admit : std::chrono::steady_clock::now(); // a group is admitted at one time
+    r.admitted = true;
+    s->active.push_back(r.id);
+    s->queue.erase(std::find(s->queue.begin(), s->queue.end(), r.id));
+    slot_jobs[r.id] = sj;
+    st.admitted++;
+    return true;
+}
 
-    // ---- plan: cancellations, admissions, prompt chunks ----------------------------------------------------------------------
-    {
-        std::lock_guard<std::mutex> lk(s->mu);
-        s->step_no++;
-        discards.swap(s->discards);
-        // a cancelled leader still forwards the prompt for its siblings; the second pass ends it once they are all cancelled too
-        for (int pass = 0; pass < 2; pass++)
-            for (size_t i = 0; i < s->active.size();) {
-                Request &r = s->reqs[s->active[i]];
-                if (r.cancel && r.siblings.empty()) finish(s, r, JL_SCHED_FINISHED, JL_FINISH_CANCELLED), st.finished++;
-                else i++;
+// must hold s->mu.  The step's plan: cancellations, admissions, and the prompt job of every prefilling request.
+static void plan(jl_sched *s, Step &p) {
+    jl_sched_stats &st = p.st;
+    std::vector<PrefillJob> &jobs = p.jobs;
+    s->step_no++;
+    p.discards.swap(s->discards);
+    // a cancelled leader still forwards the prompt for its siblings; the second pass ends it once they are all cancelled too
+    for (int pass = 0; pass < 2; pass++)
+        for (size_t i = 0; i < s->active.size();) {
+            Request &r = s->reqs[s->active[i]];
+            if (r.cancel && r.siblings.empty()) finish(s, r, JL_SCHED_FINISHED, JL_FINISH_CANCELLED), st.finished++;
+            else i++;
+        }
+    // FIFO admission.  A continuation whose parent still sits in its slot returns to that slot (always possible); every other
+    // request needs a slot from take_slot, and the first one that finds none blocks the slot-seeking requests behind it.
+    // An n-completion group is admitted whole, at its leader's place: its siblings wait behind it.
+    std::unordered_map<int64_t, SlotJob> slot_jobs; // admitted this step: request id -> slot preparation
+    bool blocked = false;
+    for (size_t qi = 0; qi < s->queue.size();) {
+        Request &r = s->reqs[s->queue[qi]];
+        if (r.leader >= 0) { // its leader is blocked
+            qi++;
+            continue;
+        }
+        for (size_t b = 0; b < r.siblings.size();) {
+            Request &sb = s->reqs[r.siblings[b]];
+            if (!sb.cancel) {
+                b++;
+                continue;
             }
-        // FIFO admission.  A continuation whose parent still sits in its slot returns to that slot (always possible); every other
-        // request needs a slot from take_slot, and the first one that finds none blocks the slot-seeking requests behind it.
-        // An n-completion group is admitted whole, at its leader's place: its siblings wait behind it.
-        bool blocked = false;
-        auto unqueue = [&](int64_t id) { s->queue.erase(std::find(s->queue.begin(), s->queue.end(), id)); };
-        for (size_t qi = 0; qi < s->queue.size();) {
-            Request &r = s->reqs[s->queue[qi]];
-            if (r.leader >= 0) { // its leader is blocked
+            s->queue.erase(std::find(s->queue.begin(), s->queue.end(), sb.id)); // behind qi
+            finish(s, sb, JL_SCHED_FINISHED, JL_FINISH_CANCELLED), st.finished++;
+        }
+        auto pa = r.parent >= 0 ? s->reqs.find(r.parent) : s->reqs.end();
+        if (!r.siblings.empty()) {
+            // all or nothing: the slots the group needs against the free slots and the kept sessions take_slot may spill
+            const int need = (int)r.siblings.size() + (pa != s->reqs.end() && pa->second.session >= 0 ? 0 : 1);
+            int avail = 0;
+            for (int k = 0; k < s->n_sessions; k++) {
+                const int64_t o = s->slot_owner[(size_t)k];
+                if (o < 0) avail++;
+                else if (s->be.offload && o != r.parent) {
+                    auto it = s->reqs.find(o);
+                    avail += it != s->reqs.end() && it->second.state == JL_SCHED_FINISHED && it->second.session == k;
+                }
+            }
+            if (blocked || need > avail) {
+                blocked = true;
                 qi++;
                 continue;
             }
-            for (size_t b = 0; b < r.siblings.size();) {
-                Request &sb = s->reqs[r.siblings[b]];
-                if (!sb.cancel) {
-                    b++;
-                    continue;
-                }
-                unqueue(sb.id); // behind qi
-                finish(s, sb, JL_SCHED_FINISHED, JL_FINISH_CANCELLED), st.finished++;
-            }
-            auto pa = r.parent >= 0 ? s->reqs.find(r.parent) : s->reqs.end();
-            if (!r.siblings.empty()) {
-                // all or nothing: the slots the group needs against the free slots and the kept sessions take_slot may spill
-                const int need = (int)r.siblings.size() + (pa != s->reqs.end() && pa->second.session >= 0 ? 0 : 1);
-                int avail = 0;
-                for (int k = 0; k < s->n_sessions; k++) {
-                    const int64_t o = s->slot_owner[(size_t)k];
-                    if (o < 0) avail++;
-                    else if (s->be.offload && o != r.parent) {
-                        auto it = s->reqs.find(o);
-                        avail += it != s->reqs.end() && it->second.state == JL_SCHED_FINISHED && it->second.session == k;
-                    }
-                }
-                if (blocked || need > avail) {
-                    blocked = true;
-                    qi++;
-                    continue;
-                }
-            }
-            if (r.cancel && r.siblings.empty()) {
-                if (pa != s->reqs.end()) pa->second.child = -1; // the parent still holds the KV and may be continued again
-                finish(s, r, JL_SCHED_FINISHED, JL_FINISH_CANCELLED), st.finished++;
-                s->queue.erase(s->queue.begin() + (long)qi);
-                continue;
-            }
-            SlotJob sj;
-            if (pa != s->reqs.end() && pa->second.session >= 0) {
-                r.session = pa->second.session; // the parent's slot with its KV; ownership moves to the continuation
-                pa->second.session = -1;
-            } else {
-                int64_t victim = -1;
-                const int slot = blocked ? -1 : take_slot(s, &victim);
-                if (slot < 0) {
-                    blocked = true;
-                    qi++;
-                    continue;
-                }
-                if (victim >= 0) {
-                    Request &v = s->reqs[victim];
-                    v.session = -1; // its KV leaves the device in this step (spill handle set when the offload returns)
-                    v.spilling = true;
-                    sj.victim = victim;
-                    st.spilled++;
-                }
-                r.session = slot;
-                if (pa != s->reqs.end()) sj.restore_from = r.parent; // continuation of a spilled session
-                else sj.reset = true;
-            }
-            if (sj.reset && s->prefix_max_pages > 0) {
-                // the longest cached whole-page prefix of the prompt that leaves its last token to forward, most recently used first
-                const int cpp = s->xb.ctx_per_page, pages = ((int)r.prompt.size() - 1) / cpp;
-                const std::vector<uint64_t> hashes = page_hashes(r.prompt.data(), pages, cpp);
-                s->pstats.lookups++;
-                for (int k = pages; k >= 1; k--) {
-                    auto e = prefix_find(s, r.prompt.data(), k, hashes[(size_t)k - 1], false);
-                    if (e == s->prefix.end()) continue;
-                    e->second.last_use = s->step_no, e->second.pins++;
-                    sj.reset = false, sj.entry = e->first, sj.handle = e->second.handle, sj.attach = k * cpp;
-                    r.prefilled = r.cached = k * cpp;
-                    break;
-                }
-            }
-            s->slot_owner[(size_t)r.session] = r.id;
-            r.state = JL_SCHED_PREFILL;
-            r.t_admit = std::chrono::steady_clock::now();
-            r.admitted = true;
-            s->active.push_back(r.id);
-            s->queue.erase(s->queue.begin() + (long)qi);
-            slot_jobs[r.id] = sj;
-            st.admitted++;
-            for (int64_t bid : r.siblings) { // the slots were counted above
-                Request &sb = s->reqs[bid];
-                SlotJob bj;
-                int64_t victim = -1;
-                sb.session = take_slot(s, &victim);
-                if (victim >= 0) {
-                    Request &v = s->reqs[victim];
-                    v.session = -1;
-                    v.spilling = true;
-                    bj.victim = victim;
-                    st.spilled++;
-                }
-                bj.reset = true;
-                s->slot_owner[(size_t)sb.session] = sb.id;
-                sb.state = JL_SCHED_PREFILL;
-                sb.t_admit = r.t_admit;
-                sb.admitted = true;
-                s->active.push_back(sb.id);
-                unqueue(sb.id);
-                slot_jobs[sb.id] = bj;
-                st.admitted++;
-            }
         }
-        int budget = s->prefill_budget > 0 ? s->prefill_budget : 0x7fffffff;
-        // the token sampled from the prompt's last row (or, for a sibling, from the forked copy of it)
-        auto first_token = [&](PrefillJob &j, Request &r) {
-            j.rng = r.rng;
-            if (r.temperature != 0.0f) j.temperature = r.temperature, j.uniform = next_uniform(r);
-            if (r.filtered()) j.top_k = r.top_k, j.top_p = r.top_p, j.filtered = true;
-            j.logprobs = r.logprobs;
-            if (r.pen.on()) j.pen = &r.pen, j.hist = r.prompt;
-        };
-        std::unordered_map<int64_t, size_t> leader_job; // group leader -> its job of this step
-        for (int64_t id : s->active) {
-            Request &r = s->reqs[id];
-            if (r.state != JL_SCHED_PREFILL) continue;
-            auto sj = slot_jobs.find(id);
-            if (r.leader >= 0) { // sibling: its slot preparation, and its first token in the step of the leader's last chunk
-                auto lj = leader_job.find(r.leader);
-                const bool last = lj != leader_job.end() && jobs[lj->second].last;
-                if (!last && sj == slot_jobs.end()) continue;
-                PrefillJob j;
-                j.id = id, j.session = r.session, j.start = 0, j.n = 0, j.pos = r.start_pos, j.last = last, j.sibling = true;
-                if (sj != slot_jobs.end()) j.slot = sj->second;
-                if (last) first_token(j, r), jobs[lj->second].sibs.push_back(jobs.size());
-                jobs.push_back(std::move(j));
-                continue;
-            }
+        if (r.cancel && r.siblings.empty()) {
+            if (pa != s->reqs.end()) pa->second.child = -1; // the parent still holds the KV and may be continued again
+            finish(s, r, JL_SCHED_FINISHED, JL_FINISH_CANCELLED), st.finished++;
+            s->queue.erase(s->queue.begin() + (long)qi);
+            continue;
+        }
+        if (!admit(s, r, !blocked, slot_jobs, st)) {
+            blocked = true;
+            qi++;
+            continue;
+        }
+        for (int64_t bid : r.siblings) admit(s, s->reqs[bid], true, slot_jobs, st); // the slots were counted above
+    }
+    int budget = s->prefill_budget > 0 ? s->prefill_budget : 0x7fffffff;
+    std::unordered_map<int64_t, size_t> leader_job; // group leader -> its job of this step
+    for (int64_t id : s->active) {
+        Request &r = s->reqs[id];
+        if (r.state != JL_SCHED_PREFILL) continue;
+        auto sj = slot_jobs.find(id);
+        PrefillJob j;
+        j.id = id, j.session = r.session, j.pos = r.start_pos + r.prefilled, j.sibling = r.leader >= 0;
+        if (sj != slot_jobs.end()) j.slot = sj->second; // the slot is prepared in the admission step even if the budget is spent
+        if (j.sibling) { // its slot preparation, and its first token in the step of the leader's last chunk
+            auto lj = leader_job.find(r.leader);
+            j.n = 0, j.last = lj != leader_job.end() && jobs[lj->second].last;
+            if (!j.last && sj == slot_jobs.end()) continue;
+            if (j.last) jobs[lj->second].sibs.push_back(jobs.size());
+        } else {
             if (budget <= 0 && sj == slot_jobs.end()) continue;
             const int left = (int)r.prompt.size() - r.prefilled;
-            const int n = left < budget ? left : (budget > 0 ? budget : 0);
-            PrefillJob j;
-            j.id = id, j.session = r.session, j.start = r.prefilled, j.n = n, j.pos = r.start_pos + r.prefilled;
-            if (sj != slot_jobs.end()) j.slot = sj->second; // the slot is prepared in the admission step even if the budget is spent
-            j.last = n > 0 && r.prefilled + n == (int)r.prompt.size();
-            if (j.last) first_token(j, r);
+            j.n = left < budget ? left : (budget > 0 ? budget : 0);
+            j.last = j.n > 0 && r.prefilled + j.n == (int)r.prompt.size();
             if (j.last && s->prefix_max_pages > 0 && r.start_pos == 0)
                 j.retain.assign(r.prompt.begin(), r.prompt.begin() + (long)(r.prompt.size() / (size_t)s->xb.ctx_per_page * (size_t)s->xb.ctx_per_page));
             j.cancelled = r.cancel;
-            j.tokens.assign(r.prompt.begin() + r.prefilled, r.prompt.begin() + r.prefilled + n);
+            j.tokens.assign(r.prompt.begin() + r.prefilled, r.prompt.begin() + r.prefilled + j.n);
             if (!r.siblings.empty()) leader_job[id] = jobs.size();
-            jobs.push_back(std::move(j));
-            budget -= n;
+            budget -= j.n;
         }
+        if (j.last) { // the token sampled from the prompt's last row (or, for a sibling, from the forked copy of it)
+            j.rng = r.rng;
+            if (r.temperature != 0.0f) j.sel.temperature = r.temperature, j.sel.uniform = next_uniform(r);
+            if (r.filtered()) j.sel.top_k = r.top_k, j.sel.top_p = r.top_p, j.sel.filtered = true;
+            j.sel.logprobs = r.logprobs;
+            if (r.pen.on()) j.sel.pen = &r.pen, j.sel.hist = r.prompt, j.sel.n_prompt = (int)r.prompt.size();
+        }
+        jobs.push_back(std::move(j));
     }
+}
 
-    // ---- backend calls, table unlocked: dropped spills, slot preparation, prompt chunks ---------------------------------------------
-    prefix_flush(s); // requests cancelled above: their KV is retained before their slots are prepared for others
-    for (int64_t h : discards) s->be.discard(s->user, h);
+// after a leader's prompt forward (table unlocked): its siblings fail with it, or get its session's KV for the prompt's positions
+static void fork_group(jl_sched *s, Step &p, size_t k) {
+    const PrefillJob &j = p.jobs[k];
+    if (j.dropped) return;
+    std::vector<int32_t> dst;
+    for (size_t b : j.sibs)
+        if (j.rc != JL_OK) p.jobs[b].rc = j.rc;
+        else if (p.jobs[b].rc == JL_OK) dst.push_back(p.jobs[b].session);
+    if (dst.empty()) return;
+    const int rc = evicting(s, [&] { return s->fb.fork(s->user, j.session, j.pos + j.n, (int)dst.size(), dst.data()); });
+    if (rc == JL_OK) return;
+    for (size_t b : j.sibs) p.jobs[b].rc = rc; // a failed fork fails the siblings only
+    std::lock_guard<std::mutex> lk(s->mu);
+    if (p.first_error == JL_OK) p.first_error = sched_error(s, rc, "request %lld: fork into %zu siblings failed (%d)", (long long)j.id, dst.size(), rc);
+}
+
+// the first tokens of completed prompts (table unlocked); without a batch backend a plain call has one row
+static int sample_first(jl_sched *s, Call &c) {
+    const int n = (int)c.sessions.size();
+    const jl_penalties pen = c.pc.get();
+    if (c.tier == PENALTY)
+        return s->pb.sample_multi_penalized(s->user, n, c.sessions.data(), c.temperatures.data(), c.top_k.data(), c.top_p.data(), c.uniforms.data(),
+                                            c.top_n.data(), &pen, c.next.data(), c.lp.data(), c.top_ids.data(), c.top_lp.data());
+    if (c.tier == LOGPROB)
+        return s->lb.sample_multi_logprobs(s->user, n, c.sessions.data(), c.temperatures.data(), c.top_k.data(), c.top_p.data(), c.uniforms.data(),
+                                           c.top_n.data(), c.next.data(), c.lp.data(), c.top_ids.data(), c.top_lp.data());
+    if (c.tier == TOPKP)
+        return s->tb.sample_multi_topkp(s->user, n, c.sessions.data(), c.temperatures.data(), c.top_k.data(), c.top_p.data(), c.uniforms.data(),
+                                        c.next.data());
+    if (s->bb.sample_multi) return s->bb.sample_multi(s->user, n, c.sessions.data(), c.temperatures.data(), c.uniforms.data(), c.next.data());
+    return s->be.sample(s->user, c.sessions[0], c.temperatures[0], c.uniforms[0], c.next.data());
+}
+
+// must hold s->mu.  The outcome of a prompt job's calls -> its request; `calls` are the first-token calls of its group.
+static void apply(jl_sched *s, Step &p, const PrefillJob &j, const std::vector<Call> &calls) {
+    jl_sched_stats &st = p.st;
+    Request &r = s->reqs[j.id];
+    if (j.sibling && r.state != JL_SCHED_PREFILL) return; // failed with its leader
+    if (j.rc != JL_OK) {
+        if (p.first_error == JL_OK) p.first_error = sched_error(s, j.rc, "request %lld: prompt forward failed (%d)", (long long)j.id, j.rc);
+        const std::vector<int64_t> sib = r.siblings; // a failed prompt fails the group
+        for (int64_t b : sib) finish(s, s->reqs[b], JL_SCHED_FAILED, JL_FINISH_ERROR), st.finished++;
+        finish(s, r, JL_SCHED_FAILED, JL_FINISH_ERROR), st.finished++;
+        return;
+    }
+    if (j.dropped) { // the prefix attach failed: the next step plans the prompt from position 0 (a sibling keeps waiting)
+        if (!j.sibling) r.prefilled = r.cached = 0;
+        if (j.last) r.rng = j.rng; // the first token is drawn again, from the same place in the stream
+        return;
+    }
+    r.prefilled += j.n;
+    st.prefill_tokens += j.n;
+    if (!j.last) return;
+    if (j.sibling) r.prefilled = (int)r.prompt.size();
+    for (int64_t b : r.siblings) s->reqs[b].leader = -1; // forked: from now on every member is an ordinary request
+    r.siblings.clear();
+    if (j.cancelled) {
+        finish(s, r, JL_SCHED_FINISHED, JL_FINISH_CANCELLED), st.finished++;
+        return;
+    }
+    const Call &c = calls[j.call];
+    r.out.push_back(c.next[j.row]);
+    if (r.logprobs >= 0) c.append_lp(r, j.row);
+    r.first_token_step = s->step_no;
+    r.t_first = std::chrono::steady_clock::now();
+    r.state = JL_SCHED_DECODING;
+    // the token sampled from the prompt is not stop-checked by the reference (AbstractModel.java:576-589)
+    check_done(s, r, false);
+    if (r.state != JL_SCHED_DECODING) st.finished++;
+}
+
+// the prompt sequence of jobs [b, e) (table unlocked): prepare their slots, ONE forward call over the chunks whose slot is ready, forks
+// and retains in job order, the first tokens of the completed prompts max_rows per call, then the outcomes.  A failed forward_multi or
+// batched first-token call is reported as the call's error; a lone job's failed call as its request's, by apply.
+static void run_group(jl_sched *s, Step &p, size_t b, size_t e) {
+    std::vector<PrefillJob> &jobs = p.jobs;
     const bool batched = s->bb.forward_multi != nullptr;
-    std::vector<int> rcs(jobs.size(), JL_OK);
-    std::vector<int32_t> first(jobs.size(), 0);
-    LpOut first_lp(jobs.size()); // a job with logprobs >= 0 gets its first token's from a logprob call
-    // the outcome of job k's calls -> its request (table locked)
-    auto apply = [&](size_t k) {
-        const PrefillJob &j = jobs[k];
-        Request &r = s->reqs[j.id];
-        if (j.sibling && r.state != JL_SCHED_PREFILL) return; // failed with its leader
-        if (rcs[k] != JL_OK) {
-            if (first_error == JL_OK) first_error = sched_error(s, rcs[k], "request %lld: prompt forward failed (%d)", (long long)j.id, rcs[k]);
-            const std::vector<int64_t> sib = r.siblings; // a failed prompt fails the group
-            for (int64_t b : sib) finish(s, s->reqs[b], JL_SCHED_FAILED, JL_FINISH_ERROR), st.finished++;
-            finish(s, r, JL_SCHED_FAILED, JL_FINISH_ERROR), st.finished++;
-            return;
-        }
-        if (j.dropped) { // the prefix attach failed: the next step plans the prompt from position 0 (a sibling keeps waiting)
-            if (!j.sibling) r.prefilled = r.cached = 0;
-            if (j.last) r.rng = j.rng; // the first token is drawn again, from the same place in the stream
-            return;
-        }
-        r.prefilled += j.n;
-        st.prefill_tokens += j.n;
-        if (j.last && j.sibling) r.prefilled = (int)r.prompt.size();
-        if (j.last) {
-            for (int64_t b : r.siblings) s->reqs[b].leader = -1; // forked: from now on every member is an ordinary request
-            r.siblings.clear();
-        }
-        if (j.last && j.cancelled) {
-            finish(s, r, JL_SCHED_FINISHED, JL_FINISH_CANCELLED), st.finished++;
-            return;
-        }
-        if (j.last) {
-            r.out.push_back(first[k]);
-            if (r.logprobs >= 0) first_lp.append_to(r, k);
-            r.first_token_step = s->step_no;
-            r.t_first = std::chrono::steady_clock::now();
-            r.state = JL_SCHED_DECODING;
-            // the token sampled from the prompt is not stop-checked by the reference (AbstractModel.java:576-589)
-            check_done(s, r, false);
-            if (r.state != JL_SCHED_DECODING) st.finished++;
-        }
-    };
-    // after the leader's prompt forward: its siblings fail with it, or get its session's KV for the prompt's positions
-    auto fork_group = [&](size_t k) {
-        const PrefillJob &j = jobs[k];
-        if (j.dropped) return;
-        std::vector<int32_t> dst;
-        for (size_t b : j.sibs)
-            if (rcs[k] != JL_OK) rcs[b] = rcs[k];
-            else if (rcs[b] == JL_OK) dst.push_back(jobs[b].session);
-        if (dst.empty()) return;
-        const int rc = evicting(s, [&] { return s->fb.fork(s->user, j.session, j.pos + j.n, (int)dst.size(), dst.data()); });
-        if (rc == JL_OK) return;
-        for (size_t b : j.sibs) rcs[b] = rc; // a failed fork fails the siblings only
-        std::lock_guard<std::mutex> lk(s->mu);
-        if (first_error == JL_OK) first_error = sched_error(s, rc, "request %lld: fork into %zu siblings failed (%d)", (long long)j.id, dst.size(), rc);
-    };
-    // siblings' slots are ready before any fork writes into them
-    for (size_t k = 0; k < jobs.size(); k++)
-        if (jobs[k].sibling) rcs[k] = prepare_slot(s, jobs[k], &first_error);
-    for (size_t k = 0; k < jobs.size(); k++) {
+    std::vector<size_t> fw; // the chunks whose slot is ready
+    std::vector<int32_t> sess, pos, len, toks;
+    for (size_t k = b; k < e; k++) {
         PrefillJob &j = jobs[k];
-        if (!j.sibling) rcs[k] = prepare_slot(s, j, &first_error);
+        if (!j.sibling) j.rc = prepare_slot(s, j, &p.first_error);
         if (j.dropped)
-            for (size_t b : j.sibs) jobs[b].dropped = true;
-        if (batched) continue;
-        // one batch_forward + sample per job, in job order
-        if (rcs[k] == JL_OK && j.n > 0 && !j.dropped)
-            rcs[k] = evicting(s, [&] { return s->be.batch_forward(s->user, j.session, j.tokens.data(), j.n, j.pos); });
-        if (!j.sibs.empty()) fork_group(k);
-        if (rcs[k] == JL_OK && !j.dropped && !j.retain.empty()) prefix_retain(s, j.session, j.retain);
-        if (rcs[k] == JL_OK && j.last && !j.cancelled && !j.dropped) {
-            const size_t W = JL_MAX_LOGPROBS;
-            if (j.pen) {
-                PenCall pc;
-                pc.add(j.pen, j.hist, (int)j.hist.size());
-                const jl_penalties pen = pc.get();
-                rcs[k] = s->pb.sample_multi_penalized(s->user, 1, &j.session, &j.temperature, &j.top_k, &j.top_p, &j.uniform, &j.logprobs, &pen,
-                                                      &first[k], &first_lp.lp[k], &first_lp.top_ids[k * W], &first_lp.top_lp[k * W]);
-            } else if (j.logprobs >= 0)
-                rcs[k] = s->lb.sample_multi_logprobs(s->user, 1, &j.session, &j.temperature, &j.top_k, &j.top_p, &j.uniform, &j.logprobs, &first[k],
-                                                     &first_lp.lp[k], &first_lp.top_ids[k * W], &first_lp.top_lp[k * W]);
-            else if (j.filtered)
-                rcs[k] = s->tb.sample_multi_topkp(s->user, 1, &j.session, &j.temperature, &j.top_k, &j.top_p, &j.uniform, &first[k]);
-            else
-                rcs[k] = s->be.sample(s->user, j.session, j.temperature, j.uniform, &first[k]);
-        }
-        std::lock_guard<std::mutex> lk(s->mu);
-        apply(k);
+            for (size_t x : j.sibs) jobs[x].dropped = true;
+        if (j.rc != JL_OK || j.n == 0 || j.dropped) continue;
+        fw.push_back(k), sess.push_back(j.session), pos.push_back(j.pos), len.push_back(j.n);
+        toks.insert(toks.end(), j.tokens.begin(), j.tokens.end());
     }
-    if (batched) {
-        // ONE forward over every chunk whose slot is ready, then the first tokens of the completed prompts, max_rows per call
-        std::vector<size_t> fw;
-        std::vector<int32_t> sess, pos, len, toks;
-        for (size_t k = 0; k < jobs.size(); k++) {
-            const PrefillJob &j = jobs[k];
-            if (rcs[k] != JL_OK || j.n == 0 || j.dropped) continue;
-            fw.push_back(k), sess.push_back(j.session), pos.push_back(j.pos), len.push_back(j.n);
-            toks.insert(toks.end(), j.tokens.begin(), j.tokens.end());
+    if (!fw.empty()) {
+        const int rc = evicting(s, [&] {
+            return batched ? s->bb.forward_multi(s->user, (int)fw.size(), sess.data(), pos.data(), len.data(), toks.data())
+                           : s->be.batch_forward(s->user, sess[0], toks.data(), len[0], pos[0]);
+        });
+        for (size_t k : fw) jobs[k].rc = rc;
+        if (rc != JL_OK && batched) {
+            std::lock_guard<std::mutex> lk(s->mu);
+            if (p.first_error == JL_OK) p.first_error = sched_error(s, rc, "prompt forward of %zu requests failed (%d)", fw.size(), rc);
         }
-        if (!fw.empty()) {
-            const int rc = evicting(s, [&] { return s->bb.forward_multi(s->user, (int)fw.size(), sess.data(), pos.data(), len.data(), toks.data()); });
-            if (rc != JL_OK) {
-                for (size_t k : fw) rcs[k] = rc;
-                std::lock_guard<std::mutex> lk(s->mu);
-                if (first_error == JL_OK) first_error = sched_error(s, rc, "prompt forward of %zu requests failed (%d)", fw.size(), rc);
-            }
-        }
-        for (size_t k = 0; k < jobs.size(); k++) {
-            if (!jobs[k].sibs.empty()) fork_group(k);
-            if (rcs[k] == JL_OK && !jobs[k].dropped && !jobs[k].retain.empty()) prefix_retain(s, jobs[k].session, jobs[k].retain);
-        }
-        std::vector<size_t> done;
-        for (size_t k = 0; k < jobs.size(); k++)
-            if (rcs[k] == JL_OK && jobs[k].last && !jobs[k].cancelled && !jobs[k].dropped) done.push_back(k);
-        for (size_t g = 0; g < done.size(); g += (size_t)s->max_rows) {
-            const size_t n = done.size() - g < (size_t)s->max_rows ? done.size() - g : (size_t)s->max_rows;
-            std::vector<int32_t> ss(n), out(n), ks(n), tn(n);
-            std::vector<float> temps(n), unis(n), ps(n);
-            bool filtered = false, logprobs = false, penalized = false;
-            PenCall pc;
-            for (size_t i = 0; i < n; i++) {
-                const PrefillJob &j = jobs[done[g + i]];
-                ss[i] = j.session, temps[i] = j.temperature, unis[i] = j.uniform, ks[i] = j.top_k, ps[i] = j.top_p, tn[i] = j.logprobs;
-                filtered = filtered || j.filtered;
-                logprobs = logprobs || j.logprobs >= 0;
-                penalized = penalized || j.pen;
-                pc.add(j.pen, j.hist, (int)j.hist.size());
-            }
-            LpOut lo(logprobs || penalized ? n : 0);
-            const jl_penalties pen = pc.get();
-            const int rc = penalized  ? s->pb.sample_multi_penalized(s->user, (int)n, ss.data(), temps.data(), ks.data(), ps.data(), unis.data(),
-                                                                     tn.data(), &pen, out.data(), lo.lp.data(), lo.top_ids.data(), lo.top_lp.data())
-                           : logprobs ? s->lb.sample_multi_logprobs(s->user, (int)n, ss.data(), temps.data(), ks.data(), ps.data(), unis.data(), tn.data(),
-                                                                    out.data(), lo.lp.data(), lo.top_ids.data(), lo.top_lp.data())
-                           : filtered ? s->tb.sample_multi_topkp(s->user, (int)n, ss.data(), temps.data(), ks.data(), ps.data(), unis.data(), out.data())
-                                      : s->bb.sample_multi(s->user, (int)n, ss.data(), temps.data(), unis.data(), out.data());
-            for (size_t i = 0; i < n; i++) rcs[done[g + i]] = rc, first[done[g + i]] = out[i];
-            for (size_t i = 0; logprobs && i < n; i++) {
-                const size_t k = done[g + i], W = JL_MAX_LOGPROBS;
-                first_lp.lp[k] = lo.lp[i];
-                std::copy(lo.top_ids.begin() + (long)(i * W), lo.top_ids.begin() + (long)((i + 1) * W), first_lp.top_ids.begin() + (long)(k * W));
-                std::copy(lo.top_lp.begin() + (long)(i * W), lo.top_lp.begin() + (long)((i + 1) * W), first_lp.top_lp.begin() + (long)(k * W));
-            }
-            if (rc != JL_OK) {
-                std::lock_guard<std::mutex> lk(s->mu);
-                if (first_error == JL_OK) first_error = sched_error(s, rc, "first-token sample of %zu requests failed (%d)", n, rc);
-            }
-        }
-        std::lock_guard<std::mutex> lk(s->mu);
-        for (size_t k = 0; k < jobs.size(); k++) apply(k);
     }
+    std::vector<size_t> done; // the completed prompts: a leader's fork has settled its siblings' status before they are reached
+    for (size_t k = b; k < e; k++) {
+        fork_group(s, p, k);
+        const PrefillJob &j = jobs[k];
+        if (j.rc == JL_OK && !j.dropped && !j.retain.empty()) prefix_retain(s, j.session, j.retain);
+        if (j.rc == JL_OK && j.last && !j.cancelled && !j.dropped) done.push_back(k);
+    }
+    std::vector<Call> calls;
+    for (size_t g = 0; g < done.size(); g += (size_t)s->max_rows) {
+        const size_t n = std::min(done.size() - g, (size_t)s->max_rows);
+        Call c(n);
+        for (size_t i = 0; i < n; i++) {
+            PrefillJob &j = jobs[done[g + i]];
+            c.add(j.session, j.sel);
+            j.call = calls.size(), j.row = i;
+        }
+        const int rc = sample_first(s, c);
+        for (size_t i = 0; i < n; i++) jobs[done[g + i]].rc = rc;
+        if (rc != JL_OK && batched) {
+            std::lock_guard<std::mutex> lk(s->mu);
+            if (p.first_error == JL_OK) p.first_error = sched_error(s, rc, "first-token sample of %zu requests failed (%d)", n, rc);
+        }
+        calls.push_back(std::move(c));
+    }
+    std::lock_guard<std::mutex> lk(s->mu);
+    for (size_t k = b; k < e; k++) apply(s, p, jobs[k], calls);
+}
 
-    // ---- one decode step for every generating request, max_rows rows per backend call ------------------------------------------------
-    std::vector<Row> rows;
+// the step's prompt jobs (table unlocked): with a batch backend one group of every job, else one group per job, in job order
+static void run_prompts(jl_sched *s, Step &p) {
+    prefix_flush(s); // requests cancelled in the plan: their KV is retained before their slots are prepared for others
+    for (int64_t h : p.discards) s->be.discard(s->user, h);
+    // siblings' slots are ready before any fork writes into them
+    for (PrefillJob &j : p.jobs)
+        if (j.sibling) j.rc = prepare_slot(s, j, &p.first_error);
+    const size_t group = s->bb.forward_multi ? p.jobs.size() : 1;
+    for (size_t b = 0; b < p.jobs.size(); b += group) run_group(s, p, b, b + group);
+}
+
+// one decode step over a call's rows (table unlocked)
+static int decode_call(jl_sched *s, Call &c) {
+    const int n = (int)c.sessions.size();
+    const jl_penalties pen = c.pc.get();
+    if (c.tier == PENALTY)
+        return s->pb.decode_penalized(s->user, n, c.sessions.data(), c.tokens.data(), c.positions.data(), c.temperatures.data(), c.top_k.data(),
+                                      c.top_p.data(), c.uniforms.data(), c.top_n.data(), &pen, c.next.data(), c.lp.data(), c.top_ids.data(),
+                                      c.top_lp.data());
+    if (c.tier == LOGPROB)
+        return s->lb.decode_logprobs(s->user, n, c.sessions.data(), c.tokens.data(), c.positions.data(), c.temperatures.data(), c.top_k.data(),
+                                     c.top_p.data(), c.uniforms.data(), c.top_n.data(), c.next.data(), c.lp.data(), c.top_ids.data(),
+                                     c.top_lp.data());
+    if (c.tier == TOPKP)
+        return s->tb.decode_topkp(s->user, n, c.sessions.data(), c.tokens.data(), c.positions.data(), c.temperatures.data(), c.top_k.data(),
+                                  c.top_p.data(), c.uniforms.data(), c.next.data());
+    return s->be.decode(s->user, n, c.sessions.data(), c.tokens.data(), c.positions.data(), c.temperatures.data(), c.uniforms.data(), c.next.data());
+}
+
+// one decode step for every generating request, max_rows rows per backend call
+static void run_decode(jl_sched *s, Step &p) {
+    jl_sched_stats &st = p.st;
+    const size_t M = (size_t)s->max_rows;
+    std::vector<Call> calls;
+    std::vector<int64_t> ids; // request of row i of call g: ids[g * max_rows + i]
     {
         std::lock_guard<std::mutex> lk(s->mu);
         for (int64_t id : s->active) {
             Request &r = s->reqs[id];
             if (r.state != JL_SCHED_DECODING) continue;
-            const float u = r.temperature != 0.0f ? next_uniform(r) : 0.0f;
-            rows.push_back(Row{id, r.session, r.out.back(), r.next_pos(), r.temperature, u, r.top_k, r.top_p, r.filtered(), r.logprobs});
+            Select x{r.temperature, r.temperature != 0.0f ? next_uniform(r) : 0.0f, r.top_k, r.top_p, r.filtered(), r.logprobs};
             if (r.pen.on()) { // the prompt, then every generated token including the one this step feeds
-                Row &w = rows.back();
-                w.pen = &r.pen, w.n_prompt = (int)r.prompt.size();
-                w.hist = r.prompt;
-                w.hist.insert(w.hist.end(), r.out.begin(), r.out.end());
+                x.pen = &r.pen, x.n_prompt = (int)r.prompt.size();
+                x.hist = r.prompt;
+                x.hist.insert(x.hist.end(), r.out.begin(), r.out.end());
             }
+            if (ids.size() % M == 0) calls.emplace_back(M);
+            Call &c = calls.back();
+            c.add(r.session, x), c.tokens.push_back(r.out.back()), c.positions.push_back(r.next_pos());
+            ids.push_back(id);
         }
     }
-    std::vector<int32_t> sess((size_t)s->max_rows), toks((size_t)s->max_rows), pos((size_t)s->max_rows), next((size_t)s->max_rows);
-    std::vector<float> temps((size_t)s->max_rows), unis((size_t)s->max_rows), ps((size_t)s->max_rows);
-    std::vector<int32_t> ks((size_t)s->max_rows), tn((size_t)s->max_rows);
-    LpOut lo((size_t)s->max_rows);
-    for (size_t g = 0; g < rows.size(); g += (size_t)s->max_rows) {
-        const int n = (int)(rows.size() - g < (size_t)s->max_rows ? rows.size() - g : (size_t)s->max_rows);
-        bool filtered = false, logprobs = false, penalized = false;
-        PenCall pc;
-        for (int i = 0; i < n; i++) {
-            const Row &w = rows[g + (size_t)i];
-            sess[(size_t)i] = w.session, toks[(size_t)i] = w.token, pos[(size_t)i] = w.position, temps[(size_t)i] = w.temperature, unis[(size_t)i] = w.uniform;
-            ks[(size_t)i] = w.top_k, ps[(size_t)i] = w.top_p, tn[(size_t)i] = w.logprobs;
-            filtered = filtered || w.filtered;
-            logprobs = logprobs || w.logprobs >= 0;
-            penalized = penalized || w.pen;
-            pc.add(w.pen, w.hist, w.n_prompt);
-        }
-        const jl_penalties pen = pc.get();
-        const int rc = evicting(s, [&] {
-            return penalized ? s->pb.decode_penalized(s->user, n, sess.data(), toks.data(), pos.data(), temps.data(), ks.data(), ps.data(), unis.data(),
-                                                      tn.data(), &pen, next.data(), lo.lp.data(), lo.top_ids.data(), lo.top_lp.data())
-                   : logprobs ? s->lb.decode_logprobs(s->user, n, sess.data(), toks.data(), pos.data(), temps.data(), ks.data(), ps.data(), unis.data(),
-                                                      tn.data(), next.data(), lo.lp.data(), lo.top_ids.data(), lo.top_lp.data())
-                   : filtered ? s->tb.decode_topkp(s->user, n, sess.data(), toks.data(), pos.data(), temps.data(), ks.data(), ps.data(), unis.data(), next.data())
-                              : s->be.decode(s->user, n, sess.data(), toks.data(), pos.data(), temps.data(), unis.data(), next.data());
-        });
+    for (size_t g = 0; g < calls.size(); g++) {
+        Call &c = calls[g];
+        const int n = (int)c.sessions.size();
+        const int rc = evicting(s, [&] { return decode_call(s, c); });
         st.decode_calls++;
         std::lock_guard<std::mutex> lk(s->mu);
         for (int i = 0; i < n; i++) {
-            Request &r = s->reqs[rows[g + i].id];
+            Request &r = s->reqs[ids[g * M + (size_t)i]];
             if (rc != JL_OK) {
-                if (first_error == JL_OK) first_error = sched_error(s, rc, "decode step of %d sessions failed (%d)", n, rc);
+                if (p.first_error == JL_OK) p.first_error = sched_error(s, rc, "decode step of %d sessions failed (%d)", n, rc);
                 finish(s, r, JL_SCHED_FAILED, JL_FINISH_ERROR), st.finished++;
                 continue;
             }
             r.forwarded++;
-            r.out.push_back(next[(size_t)i]);
-            if (r.logprobs >= 0) lo.append_to(r, (size_t)i);
+            r.out.push_back(c.next[(size_t)i]);
+            if (r.logprobs >= 0) c.append_lp(r, (size_t)i);
             st.decode_rows++;
             check_done(s, r, true);
             if (r.state != JL_SCHED_DECODING) st.finished++;
         }
     }
+}
 
-    if (s->prefix_max_pages > 0) {
-        // the step's finished requests are retained, then least recently used entries go until the cache alone holds max_pages pages
-        prefix_flush(s);
-        for (;;) {
-            int64_t only = 0;
-            if (s->xb.retained(s->user, nullptr, &only) != JL_OK) break;
-            {
-                std::lock_guard<std::mutex> lk(s->mu);
-                s->pstats.pages_retained_only = only;
-            }
-            if (only <= s->prefix_max_pages || !prefix_evict(s)) break;
+// the step's finished requests are retained, then least recently used entries go until the cache alone holds max_pages pages
+static void prefix_upkeep(jl_sched *s) {
+    if (s->prefix_max_pages <= 0) return;
+    prefix_flush(s);
+    for (;;) {
+        int64_t only = 0;
+        if (s->xb.retained(s->user, nullptr, &only) != JL_OK) break;
+        {
+            std::lock_guard<std::mutex> lk(s->mu);
+            s->pstats.pages_retained_only = only;
         }
+        if (only <= s->prefix_max_pages || !prefix_evict(s)) break;
     }
+}
+
+// the counts of `st` added to `sum`; active and queued are levels, taken as they are
+static void add_stats(jl_sched_stats &sum, const jl_sched_stats &st) {
+    sum.admitted += st.admitted, sum.prefill_tokens += st.prefill_tokens, sum.decode_rows += st.decode_rows;
+    sum.decode_calls += st.decode_calls, sum.finished += st.finished, sum.spilled += st.spilled;
+    sum.active = st.active, sum.queued = st.queued;
+}
+
+// the levels after the step, and the step's counts added to the scheduler's totals
+static void record_stats(jl_sched *s, jl_sched_stats &st) {
+    std::lock_guard<std::mutex> lk(s->mu);
+    st.active = (int)s->active.size();
+    st.queued = (int)s->queue.size();
+    add_stats(s->totals, st);
+}
+
+extern "C" int jl_sched_step(jl_sched *s, jl_sched_stats *stats) {
+    if (!s) return JL_ERR_INVALID;
+    std::lock_guard<std::mutex> step_lock(s->step_mu);
+    Step p;
     {
         std::lock_guard<std::mutex> lk(s->mu);
-        st.active = (int)s->active.size();
-        st.queued = (int)s->queue.size();
-        s->totals.admitted += st.admitted, s->totals.prefill_tokens += st.prefill_tokens, s->totals.decode_rows += st.decode_rows;
-        s->totals.decode_calls += st.decode_calls, s->totals.finished += st.finished, s->totals.spilled += st.spilled;
-        s->totals.active = st.active, s->totals.queued = st.queued;
+        plan(s, p);
     }
-    if (stats) *stats = st;
-    return first_error;
+    run_prompts(s, p);
+    run_decode(s, p);
+    prefix_upkeep(s);
+    record_stats(s, p.st);
+    if (stats) *stats = p.st;
+    return p.first_error;
 }
 
 extern "C" int jl_sched_run(jl_sched *s, int max_steps, jl_sched_stats *totals) {
@@ -1357,8 +1354,7 @@ extern "C" int jl_sched_run(jl_sched *s, int max_steps, jl_sched_stats *totals) 
         jl_sched_stats st;
         const int rc = jl_sched_step(s, &st);
         if (rc != JL_OK && rc_all == JL_OK) rc_all = rc;
-        sum.admitted += st.admitted, sum.prefill_tokens += st.prefill_tokens, sum.decode_rows += st.decode_rows;
-        sum.decode_calls += st.decode_calls, sum.finished += st.finished, sum.spilled += st.spilled, sum.active = st.active, sum.queued = st.queued;
+        add_stats(sum, st);
         if (st.active == 0 && st.queued == 0) break;
         // nothing admitted, forwarded or decoded although work is queued: every slot is held by a kept session
         if (st.admitted == 0 && st.prefill_tokens == 0 && st.decode_rows == 0 && st.finished == 0) {
