@@ -29,11 +29,6 @@ __device__ __forceinline__ uint32_t pa_pack(float lo, float hi) {
     __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
     return *reinterpret_cast<uint32_t *>(&v);
 }
-__device__ __forceinline__ void pa_mma(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 __device__ __forceinline__ void pa_ldsm4(uint32_t (&r)[4], uint32_t addr) {
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
 }
@@ -177,8 +172,8 @@ __device__ __forceinline__ void prefill_attention_body(const AttnParams &p, int 
             for (int nt = 0; nt < PA_KT / 8; nt += 2) {
                 uint32_t b[4]; // (nt, k lo) (nt, k hi) (nt+1, k lo) (nt+1, k hi)
                 pa_ldsm4(b, ks_base + (uint32_t)((((nt + (lm >> 1)) * 8 + lr) * LDS + ks * 16 + (lm & 1) * 8) * 2));
-                pa_mma(s[nt], qf[ks], b[0], b[1]);
-                pa_mma(s[nt + 1], qf[ks], b[2], b[3]);
+                mma_bf16(s[nt], qf[ks], b[0], b[1]);
+                mma_bf16(s[nt + 1], qf[ks], b[2], b[3]);
             }
         }
         // ---- scale, causal mask, online softmax ---------------------------------------------------------------
@@ -222,8 +217,8 @@ __device__ __forceinline__ void prefill_attention_body(const AttnParams &p, int 
             for (int nt = 0; nt < HS / 8; nt += 2) {
                 uint32_t b[4]; // (k lo, nt) (k hi, nt) (k lo, nt+1) (k hi, nt+1)
                 pa_ldsm4t(b, vs_base + (uint32_t)(((j * 16 + (lm & 1) * 8 + lr) * LDS + (nt + (lm >> 1)) * 8) * 2));
-                pa_mma(o[nt], pf[j], b[0], b[1]);
-                pa_mma(o[nt + 1], pf[j], b[2], b[3]);
+                mma_bf16(o[nt], pf[j], b[0], b[1]);
+                mma_bf16(o[nt + 1], pf[j], b[2], b[3]);
             }
         }
     }

@@ -422,6 +422,80 @@ __device__ __forceinline__ float ldg_stream_f32(const float *p, unsigned long lo
     asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(r) : "l"(p), "l"(pol));
     return r;
 }
+
+// ---- tensor-core MMAs and cp.async (decode GEMMs, prefill attention) ----
+// c += a (16x32, row) * b (32x8, col): u8 x s8 (Q4 nibbles) and s8 x s8 (Q8_0) -> s32
+__device__ __forceinline__ void mma_u8s8(int (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.u8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
+                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void mma_s8s8(int (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
+                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+// d += a (16x16, row) * b (16x8, col): bf16 x bf16 -> f32
+__device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+// 16-byte global -> shared copy, with an L2 cache policy or the default one
+__device__ __forceinline__ void cp16(uint32_t dst, const void *src, unsigned long long pol) {
+    asm volatile("cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void cp16(uint32_t dst, const void *src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+// wait until at most `pending` of this thread's copy groups are still in flight
+__device__ __forceinline__ void cp_wait(int pending) {
+    switch (pending) {
+        case 0: asm volatile("cp.async.wait_group 0;" ::: "memory"); break;
+        case 1: asm volatile("cp.async.wait_group 1;" ::: "memory"); break;
+        case 2: asm volatile("cp.async.wait_group 2;" ::: "memory"); break;
+        case 3: asm volatile("cp.async.wait_group 3;" ::: "memory"); break;
+        default: asm volatile("cp.async.wait_group 4;" ::: "memory"); break;
+    }
+}
+
+// One pipeline stage of a 16-row weight strip (jl_gemm8.cu, jl_gemm64.cu): a 128-byte chunk of each of the 16 rows, then the
+// rows' block scales.  The row stride 128 + 16 makes the fragment loads conflict free (lane (g, t) reads word g*36 + 4u + t:
+// 32 distinct banks).  ROWB and SC_OFF are the same for both weight types, and so is the stage size.
+#define STRIP_STAGE 3072 // bytes of one strip stage: 16 rows x 144 B of weights + 16 rows x <= 48 B of block scales
+template <int WDT>
+struct Strip {
+    static constexpr int BPC = WDT == JL_Q4 ? 8 : 4;  // blocks per 128-byte row chunk
+    static constexpr int BB = WDT == JL_Q4 ? 16 : 32; // weight bytes per block
+    static constexpr int SCS = BPC * 4 + 16;          // staged scale row stride (bytes)
+    static constexpr int ROWB = 144;                  // staged weight row stride (bytes)
+    static constexpr int SC_OFF = 16 * ROWB;          // scales behind the 16 weight rows
+};
+
+// One warp issues stage `st` of a strip: the 128-byte chunk at block column cb of weight rows p.row0 + local0 + 0..15 of tensor
+// (wb, wsb) (8 lanes per row, 4 copies per lane) and their scales.  Rows at or past rows_left do not exist and copy the strip's
+// first row instead (their results are never stored).
+template <int WDT>
+__device__ __forceinline__ void strip_stage(uint32_t st, const GemvParams &p, const void *wb, const float *wsb, int local0, int rows_left,
+                                            size_t ldb, size_t cb, int lane, unsigned long long pol) {
+    using S = Strip<WDT>;
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        const int r = (lane >> 3) + 4 * i, rl = r < rows_left ? r : 0;
+        const size_t blk0 = (size_t)(p.row0 + local0 + rl) * ldb + cb;
+        cp16(st + r * S::ROWB + (lane & 7) * 16, (const uint8_t *)wb + blk0 * S::BB + (lane & 7) * 16, pol);
+    }
+    if (WDT == JL_Q4) { // 16 rows x 32 B of scales: two lanes per row
+        const int r = lane >> 1, rl = r < rows_left ? r : 0;
+        const size_t blk0 = (size_t)(p.row0 + local0 + rl) * ldb + cb;
+        cp16(st + S::SC_OFF + r * S::SCS + (lane & 1) * 16, wsb + blk0 + (lane & 1) * 4, pol);
+    } else if (lane < 16) { // 16 rows x 16 B
+        const int r = lane, rl = r < rows_left ? r : 0;
+        const size_t blk0 = (size_t)(p.row0 + local0 + rl) * ldb + cb;
+        cp16(st + S::SC_OFF + r * S::SCS, wsb + blk0, pol);
+    }
+}
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
     unsigned long long t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));

@@ -23,37 +23,10 @@
 
 #define G64_WARPS 8
 #define G64_THREADS (G64_WARPS * 32)
-#define G64_ROWB 144 // staged weight row stride: 128 + 16 (conflict-free fragment loads, as G8_ROWB)
-#define G64_SC_OFF (16 * G64_ROWB)
-#define G64_WSTAGE 3072 // one warp's weights of one tensor in one stage: 16 rows x 144 B + 16 rows x <= 48 B of block scales
 #define G64_MAX_STAGES 6
 #define G64_SMEM_LIMIT (227 * 1024)
 #define G64_MAGIC 0x4B400000 // float bits of 1.5 * 2^23
 
-template <int WDT>
-struct G64Cfg {
-    static constexpr int BPC = WDT == JL_Q4 ? 8 : 4;  // blocks per 128-byte weight row chunk
-    static constexpr int BB = WDT == JL_Q4 ? 16 : 32; // weight bytes per block
-    static constexpr int SCS = BPC * 4 + 16;          // staged weight scale row stride (bytes)
-    static constexpr int KC = BPC * 32;               // K elements per stage
-    static constexpr int AST = KC + 16;               // staged activation row stride (bytes)
-};
-
-__device__ __forceinline__ void g64_mma_u8s8(int (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.u8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
-                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void g64_mma_s8s8(int (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
-                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void g64_mma_bf16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 // two nibbles (bytes `sel` of x, each 0..15) -> BF16x2 of (nibble - 8), exact: 0x4300 | n is the BF16 128 + n
 __device__ __forceinline__ uint32_t g64_nib2bf(uint32_t x, uint32_t sel) {
     const uint32_t v = __byte_perm(x, 0, sel) | 0x43004300u;
@@ -64,22 +37,6 @@ __device__ __forceinline__ uint32_t g64_nib2bf(uint32_t x, uint32_t sel) {
 __device__ __forceinline__ uint32_t g64_s82bf(uint32_t w, int h) {
     const __nv_bfloat162 r = __floats2bfloat162_rn((float)(int8_t)(w >> (16 * h)), (float)(int8_t)(w >> (16 * h + 8)));
     return *(const uint32_t *)&r;
-}
-__device__ __forceinline__ void g64_cp16(uint32_t dst, const void *src, unsigned long long pol) {
-    asm volatile("cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "l"(pol) : "memory");
-}
-__device__ __forceinline__ void g64_cp16_plain(uint32_t dst, const void *src) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-}
-__device__ __forceinline__ void g64_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void g64_wait(int pending) {
-    switch (pending) {
-        case 0: asm volatile("cp.async.wait_group 0;" ::: "memory"); break;
-        case 1: asm volatile("cp.async.wait_group 1;" ::: "memory"); break;
-        case 2: asm volatile("cp.async.wait_group 2;" ::: "memory"); break;
-        case 3: asm volatile("cp.async.wait_group 3;" ::: "memory"); break;
-        default: asm volatile("cp.async.wait_group 4;" ::: "memory"); break;
-    }
 }
 
 // ---- prologue: (RMSNorm) + Q8 quantisation, one CTA per padded row ----------------------------------------------------------
@@ -201,9 +158,12 @@ template <int WDT, int EPI, int NT, bool FA>
 __global__ void __launch_bounds__(G64_THREADS, 1) gemm64_kernel(const GemvParams p, const int nst, const int ks) {
     extern __shared__ __align__(16) unsigned char smem[];
     constexpr int NW = EPI == EPI_SILU_MUL ? 2 : 1;
-    constexpr int BPC = G64Cfg<WDT>::BPC, BB = G64Cfg<WDT>::BB, SCS = G64Cfg<WDT>::SCS, KC = G64Cfg<WDT>::KC, AST = G64Cfg<WDT>::AST;
+    using S = Strip<WDT>;
+    constexpr int BPC = S::BPC, SCS = S::SCS;
+    constexpr int KC = BPC * 32;  // K elements per stage
+    constexpr int AST = KC + 16;  // staged activation row stride (bytes)
     constexpr int MP = NT * 8; // padded rows
-    constexpr int W_BYTES = G64_WARPS * NW * G64_WSTAGE, A_BYTES = FA ? 0 : MP * AST, S_BYTES = FA ? 0 : BPC * MP * 8;
+    constexpr int W_BYTES = G64_WARPS * NW * STRIP_STAGE, A_BYTES = FA ? 0 : MP * AST, S_BYTES = FA ? 0 : BPC * MP * 8;
     constexpr int STAGE = W_BYTES + A_BYTES + S_BYTES;
     constexpr int UNROLL_U = NW * NT >= 12 ? 1 : BPC; // gate+up at 48 / 64 rows: 48 / 64 accumulators; a full unroll spills
     __shared__ int last_sh;
@@ -250,39 +210,23 @@ __global__ void __launch_bounds__(G64_THREADS, 1) gemm64_kernel(const GemvParams
             if (have) {
                 const size_t cb = (size_t)(p.w_col_off / 32) + (size_t)c * BPC;
 #pragma unroll
-                for (int w = 0; w < NW; w++) {
-                    const uint32_t ws = st + (uint32_t)(warp * NW + w) * G64_WSTAGE;
-#pragma unroll
-                    for (int i = 0; i < 4; i++) {
-                        const int r = (lane >> 3) + 4 * i, rl = r < rows_left ? r : 0;
-                        const size_t blk0 = (size_t)(p.row0 + local0[w] + rl) * ldb + cb;
-                        g64_cp16(ws + r * G64_ROWB + (lane & 7) * 16, (const uint8_t *)wb[w] + blk0 * BB + (lane & 7) * 16, pol);
-                    }
-                    if (WDT == JL_Q4) { // 16 rows x 32 B of scales: two lanes per row
-                        const int r = lane >> 1, rl = r < rows_left ? r : 0;
-                        const size_t blk0 = (size_t)(p.row0 + local0[w] + rl) * ldb + cb;
-                        g64_cp16(ws + G64_SC_OFF + r * SCS + (lane & 1) * 16, wsb[w] + blk0 + (lane & 1) * 4, pol);
-                    } else if (lane < 16) { // 16 rows x 16 B
-                        const int r = lane, rl = r < rows_left ? r : 0;
-                        const size_t blk0 = (size_t)(p.row0 + local0[w] + rl) * ldb + cb;
-                        g64_cp16(ws + G64_SC_OFF + r * SCS, wsb[w] + blk0, pol);
-                    }
-                }
+                for (int w = 0; w < NW; w++)
+                    strip_stage<WDT>(st + (uint32_t)(warp * NW + w) * STRIP_STAGE, p, wb[w], wsb[w], local0[w], rows_left, ldb, cb, lane, pol);
             }
             if (FA) {
-                g64_commit();
+                cp_commit();
                 return;
             }
             // activations of every row for this K-slice (L2 hits; default policy keeps them there for the other CTAs)
             const uint32_t as = st + W_BYTES;
             for (int i = tid; i < MP * (KC / 16); i += G64_THREADS) {
                 const int r = i / (KC / 16), o = (i - r * (KC / 16)) * 16;
-                g64_cp16_plain(as + r * AST + o, act + (size_t)r * K + (size_t)c * KC + o);
+                cp16(as + r * AST + o, act + (size_t)r * K + (size_t)c * KC + o);
             }
             const uint32_t ss = as + A_BYTES;
-            for (int i = tid; i < S_BYTES / 16; i += G64_THREADS) g64_cp16_plain(ss + i * 16, act_s + (size_t)c * S_BYTES + (size_t)i * 16);
+            for (int i = tid; i < S_BYTES / 16; i += G64_THREADS) cp16(ss + i * 16, act_s + (size_t)c * S_BYTES + (size_t)i * 16);
         }
-        g64_commit();
+        cp_commit();
     };
     for (int i = 0; i < nst - 1; i++) issue(i);
 
@@ -298,12 +242,12 @@ __global__ void __launch_bounds__(G64_THREADS, 1) gemm64_kernel(const GemvParams
     // operands: lane t supplies elements 4t..4t+3 (first MMA) and 16+4t..19+4t (second), k-slots 2t, 2t+1, 2t+8, 2t+9 of each.
     const uint16_t *fa_act = (const uint16_t *)p.wide_act;
     auto fa_chunk = [&](const unsigned char *st, int c) {
-        const unsigned char *ws = st + warp * G64_WSTAGE; // NW == 1
+        const unsigned char *ws = st + warp * STRIP_STAGE; // NW == 1
 #pragma unroll 1
         for (int u = 0; u < BPC; u++) {
             uint32_t A[2][4];
             if (WDT == JL_Q4) {
-                const uint32_t w0 = *(const uint32_t *)(ws + g * G64_ROWB + u * 16 + 4 * t), w1 = *(const uint32_t *)(ws + (g + 8) * G64_ROWB + u * 16 + 4 * t);
+                const uint32_t w0 = *(const uint32_t *)(ws + g * S::ROWB + u * 16 + 4 * t), w1 = *(const uint32_t *)(ws + (g + 8) * S::ROWB + u * 16 + 4 * t);
 #pragma unroll
                 for (int h = 0; h < 2; h++) {
                     const uint32_t x0 = (w0 >> (4 * h)) & 0x0F0F0F0Fu, x1 = (w1 >> (4 * h)) & 0x0F0F0F0Fu;
@@ -312,12 +256,12 @@ __global__ void __launch_bounds__(G64_THREADS, 1) gemm64_kernel(const GemvParams
             } else {
 #pragma unroll
                 for (int h = 0; h < 2; h++) {
-                    const uint32_t w0 = *(const uint32_t *)(ws + g * G64_ROWB + u * 32 + 16 * h + 4 * t);
-                    const uint32_t w1 = *(const uint32_t *)(ws + (g + 8) * G64_ROWB + u * 32 + 16 * h + 4 * t);
+                    const uint32_t w0 = *(const uint32_t *)(ws + g * S::ROWB + u * 32 + 16 * h + 4 * t);
+                    const uint32_t w1 = *(const uint32_t *)(ws + (g + 8) * S::ROWB + u * 32 + 16 * h + 4 * t);
                     A[h][0] = g64_s82bf(w0, 0), A[h][1] = g64_s82bf(w1, 0), A[h][2] = g64_s82bf(w0, 1), A[h][3] = g64_s82bf(w1, 1);
                 }
             }
-            const float sw0 = *(const float *)(ws + G64_SC_OFF + g * SCS + u * 4), sw1 = *(const float *)(ws + G64_SC_OFF + (g + 8) * SCS + u * 4);
+            const float sw0 = *(const float *)(ws + S::SC_OFF + g * SCS + u * 4), sw1 = *(const float *)(ws + S::SC_OFF + (g + 8) * SCS + u * 4);
             const size_t e = (size_t)c * KC + u * 32 + 4 * t;
 #pragma unroll
             for (int j = 0; j < NT; j++) {
@@ -327,8 +271,8 @@ __global__ void __launch_bounds__(G64_THREADS, 1) gemm64_kernel(const GemvParams
                 for (int P = 2; P >= 0; P--) {
                     const uint16_t *pp = ar + (size_t)P * MP * K;
                     const uint2 b0 = __ldg((const uint2 *)pp), b1 = __ldg((const uint2 *)(pp + 16));
-                    g64_mma_bf16(cf, A[0], b0.x, b0.y);
-                    g64_mma_bf16(cf, A[1], b1.x, b1.y);
+                    mma_bf16(cf, A[0], b0.x, b0.y);
+                    mma_bf16(cf, A[1], b1.x, b1.y);
                 }
                 acc[0][j][0] = fmaf(sw0, cf[0], acc[0][j][0]);
                 acc[0][j][1] = fmaf(sw0, cf[1], acc[0][j][1]);
@@ -339,7 +283,7 @@ __global__ void __launch_bounds__(G64_THREADS, 1) gemm64_kernel(const GemvParams
     };
 
     for (int q = 0; q < cpk; q++) {
-        g64_wait(nst - 2); // this thread's copies of stage q have landed ...
+        cp_wait(nst - 2); // this thread's copies of stage q have landed ...
         __syncthreads();   // ... and every thread's; all threads are also done with stage q - 1, which the next issue overwrites
         issue(q + nst - 1);
         if (!have) continue;
@@ -351,25 +295,25 @@ __global__ void __launch_bounds__(G64_THREADS, 1) gemm64_kernel(const GemvParams
         const unsigned char *as = st + W_BYTES, *ss = as + A_BYTES;
 #pragma unroll
         for (int w = 0; w < NW; w++) {
-            const unsigned char *ws = st + (warp * NW + w) * G64_WSTAGE;
+            const unsigned char *ws = st + (warp * NW + w) * STRIP_STAGE;
 #pragma unroll(UNROLL_U)
             for (int u = 0; u < BPC; u++) {
                 uint32_t a0, a1, a2, a3;
                 if (WDT == JL_Q4) {
                     // bytes [4t, 4t+4) of a block: low nibbles = elements 4t..4t+3, high nibbles = elements 16+4t..19+4t
-                    const uint32_t w0 = *(const uint32_t *)(ws + g * G64_ROWB + u * 16 + 4 * t), w1 = *(const uint32_t *)(ws + (g + 8) * G64_ROWB + u * 16 + 4 * t);
+                    const uint32_t w0 = *(const uint32_t *)(ws + g * S::ROWB + u * 16 + 4 * t), w1 = *(const uint32_t *)(ws + (g + 8) * S::ROWB + u * 16 + 4 * t);
                     a0 = w0 & 0x0F0F0F0Fu, a1 = w1 & 0x0F0F0F0Fu, a2 = (w0 >> 4) & 0x0F0F0F0Fu, a3 = (w1 >> 4) & 0x0F0F0F0Fu;
                 } else {
-                    const unsigned char *r0p = ws + g * G64_ROWB + u * 32 + 4 * t, *r1p = ws + (g + 8) * G64_ROWB + u * 32 + 4 * t;
+                    const unsigned char *r0p = ws + g * S::ROWB + u * 32 + 4 * t, *r1p = ws + (g + 8) * S::ROWB + u * 32 + 4 * t;
                     a0 = *(const uint32_t *)r0p, a1 = *(const uint32_t *)r1p, a2 = *(const uint32_t *)(r0p + 16), a3 = *(const uint32_t *)(r1p + 16);
                 }
-                const float sw0 = *(const float *)(ws + G64_SC_OFF + g * SCS + u * 4), sw1 = *(const float *)(ws + G64_SC_OFF + (g + 8) * SCS + u * 4);
+                const float sw0 = *(const float *)(ws + S::SC_OFF + g * SCS + u * 4), sw1 = *(const float *)(ws + S::SC_OFF + (g + 8) * SCS + u * 4);
 #pragma unroll
                 for (int j = 0; j < NT; j++) {
                     const uint2 bf = *(const uint2 *)(as + (8 * j + g) * AST + u * 32 + 8 * t);
                     int c[4] = {0, 0, 0, 0};
-                    if (WDT == JL_Q4) g64_mma_u8s8(c, a0, a1, a2, a3, bf.x, bf.y);
-                    else g64_mma_s8s8(c, a0, a1, a2, a3, bf.x, bf.y);
+                    if (WDT == JL_Q4) mma_u8s8(c, a0, a1, a2, a3, bf.x, bf.y);
+                    else mma_s8s8(c, a0, a1, a2, a3, bf.x, bf.y);
                     // c[0] = (row g, session 8j+2t), c[1] = (row g, 8j+2t+1), c[2] = (row g+8, 8j+2t), c[3] = (row g+8, 8j+2t+1)
                     const uint4 s = *(const uint4 *)(ss + ((size_t)u * MP + 8 * j + 2 * t) * 8);
                     const float sa0 = __uint_as_float(s.x), sa1 = __uint_as_float(s.z);
@@ -383,7 +327,7 @@ __global__ void __launch_bounds__(G64_THREADS, 1) gemm64_kernel(const GemvParams
             }
         }
     }
-    g64_wait(0);
+    cp_wait(0);
 
     if (ks > 1) {
         // split-K: publish this CTA's tile; the last CTA of the group adds all tiles in split order
@@ -453,7 +397,7 @@ static int g64_nt(int M) { return M <= 16 ? 2 : (M <= 32 ? 4 : (M <= 48 ? 6 : 8)
 static bool g64_fa(int prologue) { return prologue == PRO_F32 || prologue == PRO_RMSNORM_F32; }
 static size_t g64_stage(int wdt, int epi, int nt, bool fa) {
     const int bpc = wdt == JL_Q4 ? 8 : 4, kc = bpc * 32, nw = epi == EPI_SILU_MUL ? 2 : 1;
-    return (size_t)G64_WARPS * nw * G64_WSTAGE + (fa ? 0 : (size_t)nt * 8 * (kc + 16) + (size_t)bpc * nt * 8 * 8);
+    return (size_t)G64_WARPS * nw * STRIP_STAGE + (fa ? 0 : (size_t)nt * 8 * (kc + 16) + (size_t)bpc * nt * 8 * 8);
 }
 static int g64_stages(int wdt, int epi, int nt, bool fa) {
     const int n = (int)((G64_SMEM_LIMIT - 1024) / g64_stage(wdt, epi, nt, fa));

@@ -18,46 +18,8 @@
 
 #define G8_MAX_WARPS 16
 #define G8_PAD 16        // bytes added to a session's activation row in shared memory: makes the fragment loads bank-conflict free
-#define G8_CHUNK 128     // weight bytes of one row in one pipeline stage (8 Q4 blocks / 4 I8 blocks)
-#define G8_ROWB 144      // staged row stride: 128 + 16 (lane (g, t) reads word g*36 + 4u + t: 32 distinct banks)
-#define G8_SC_OFF (16 * G8_ROWB)
-#define G8_STAGE 3072    // 16 rows x 144 B of weights + 16 rows x <= 48 B of block scales
 #define G8_MAX_STAGES 6
 #define G8_SMEM_LIMIT (227 * 1024)
-
-__device__ __forceinline__ void mma_u8s8(int (&c)[4], const uint32_t a0, const uint32_t a1, const uint32_t a2, const uint32_t a3, const uint32_t b0,
-                                         const uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.u8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
-                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void mma_s8s8(int (&c)[4], const uint32_t a0, const uint32_t a1, const uint32_t a2, const uint32_t a3, const uint32_t b0,
-                                         const uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
-                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void g8_cp16(uint32_t dst, const void *src, unsigned long long pol) {
-    asm volatile("cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "l"(pol) : "memory");
-}
-__device__ __forceinline__ void g8_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-// wait until at most `pending` of this thread's copy groups are still in flight
-__device__ __forceinline__ void g8_wait(int pending) {
-    switch (pending) {
-        case 0: asm volatile("cp.async.wait_group 0;" ::: "memory"); break;
-        case 1: asm volatile("cp.async.wait_group 1;" ::: "memory"); break;
-        case 2: asm volatile("cp.async.wait_group 2;" ::: "memory"); break;
-        case 3: asm volatile("cp.async.wait_group 3;" ::: "memory"); break;
-        default: asm volatile("cp.async.wait_group 4;" ::: "memory"); break;
-    }
-}
-
-template <int WDT>
-struct G8Cfg {
-    static constexpr int BPC = WDT == JL_Q4 ? 8 : 4;  // blocks per 128-byte row chunk
-    static constexpr int BB = WDT == JL_Q4 ? 16 : 32; // bytes per block
-    static constexpr int SCS = BPC * 4 + 16;          // staged scale row stride (bytes)
-};
 
 // first weight/scale block of (strip, sub-tensor w) rows; all 16 rows of a strip lie in one tensor (jl_gemm8_supported)
 template <int NW>
@@ -88,7 +50,8 @@ __global__ void __launch_bounds__(NWARP * 32, 1) gemm8_kernel(const GemvParams p
     extern __shared__ __align__(16) unsigned char smem[];
     constexpr bool NORM = PRO == PRO_RMSNORM_QUANT;
     constexpr int NW = EPI == EPI_SILU_MUL ? 2 : 1;
-    constexpr int BPC = G8Cfg<WDT>::BPC, BB = G8Cfg<WDT>::BB, SCS = G8Cfg<WDT>::SCS;
+    using S = Strip<WDT>;
+    constexpr int BPC = S::BPC, SCS = S::SCS;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int g = lane >> 2, t = lane & 3;
     const int K = p.K, nblk = K / 32, M = p.M;
@@ -96,7 +59,7 @@ __global__ void __launch_bounds__(NWARP * 32, 1) gemm8_kernel(const GemvParams p
     int8_t *aq = (int8_t *)smem;                          // [8][astride]
     const int sst = nblk + 1;                             // scale / sum row stride (+1: the sessions a lane group reads hit different banks)
     uint2 *ass = (uint2 *)(smem + (size_t)8 * astride);   // [8][sst] {scale bits, block sum}
-    unsigned char *stages = (unsigned char *)(ass + (size_t)8 * sst) + (size_t)warp * nst * G8_STAGE;
+    unsigned char *stages = (unsigned char *)(ass + (size_t)8 * sst) + (size_t)warp * nst * STRIP_STAGE;
     const uint32_t stages_u32 = (uint32_t)__cvta_generic_to_shared(stages);
     __shared__ double red_sh[G8_WARPS][8];
     __shared__ float rs_sh[8];
@@ -125,33 +88,18 @@ __global__ void __launch_bounds__(NWARP * 32, 1) gemm8_kernel(const GemvParams p
             const float *wsb;
             int local0;
             g8_strip_base<NW>(p, p_strip, p_w, wb, wsb, local0);
-            const uint32_t st = stages_u32 + (uint32_t)(p_q % nst) * G8_STAGE;
+            const uint32_t st = stages_u32 + (uint32_t)(p_q % nst) * STRIP_STAGE;
             const int rows_left = p.total_rows - p_strip * 16; // rows of this strip that exist (>= 1)
             const size_t ldb = (size_t)(p.ldw / 32);
             const size_t cb = (size_t)(p.w_col_off / 32) + (size_t)(part * cpp + p_c) * BPC;
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                const int r = (lane >> 3) + 4 * i;
-                const int rl = r < rows_left ? r : 0;
-                const size_t blk0 = (size_t)(p.row0 + local0 + rl) * ldb + cb;
-                g8_cp16(st + r * G8_ROWB + (lane & 7) * 16, (const uint8_t *)wb + blk0 * BB + (lane & 7) * 16, pol);
-            }
-            if (WDT == JL_Q4) { // 16 rows x 32 B of scales: two lanes per row
-                const int r = lane >> 1, rl = r < rows_left ? r : 0;
-                const size_t blk0 = (size_t)(p.row0 + local0 + rl) * ldb + cb;
-                g8_cp16(st + G8_SC_OFF + r * SCS + (lane & 1) * 16, wsb + blk0 + (lane & 1) * 4, pol);
-            } else if (lane < 16) { // 16 rows x 16 B
-                const int r = lane, rl = r < rows_left ? r : 0;
-                const size_t blk0 = (size_t)(p.row0 + local0 + rl) * ldb + cb;
-                g8_cp16(st + G8_SC_OFF + r * SCS, wsb + blk0, pol);
-            }
+            strip_stage<WDT>(st, p, wb, wsb, local0, rows_left, ldb, cb, lane, pol);
             if (++p_c == cpp) {
                 p_c = 0;
                 if (++p_w == NW) p_w = 0, p_strip += rstride;
             }
         }
         p_q++;
-        g8_commit();
+        cp_commit();
     };
     for (int i = 0; i < nst - 1; i++) issue();
 
@@ -260,7 +208,7 @@ __global__ void __launch_bounds__(NWARP * 32, 1) gemm8_kernel(const GemvParams p
 
     // ---- main loop: rounds of (strip, tensor, chunk) tasks ----
     const int8_t *arow = aq + (size_t)g * astride; // this lane's session (B fragment column n = g)
-    float *red = (float *)(stages - (size_t)warp * nst * G8_STAGE + (size_t)G8_WARPS * nst * G8_STAGE); // [2][8 warps][NW][4][32]
+    float *red = (float *)(stages - (size_t)warp * nst * STRIP_STAGE + (size_t)G8_WARPS * nst * STRIP_STAGE); // [2][8 warps][NW][4][32]
     int q = 0;
     for (int r = 0; r < rounds; r++) {
         const int strip = strip0 + r * rstride;
@@ -274,10 +222,10 @@ __global__ void __launch_bounds__(NWARP * 32, 1) gemm8_kernel(const GemvParams p
 #pragma unroll
             for (int w = 0; w < NW; w++) {
                 for (int cc = 0; cc < cpp; cc++, q++) {
-                    g8_wait(nst - 2); // task q has landed (for this lane's copies) ...
+                    cp_wait(nst - 2); // task q has landed (for this lane's copies) ...
                     __syncwarp();     // ... and for every lane's; all lanes are also done with task q - 1, whose stage the next issue overwrites
                     issue();
-                    const unsigned char *st = stages + (size_t)(q % nst) * G8_STAGE;
+                    const unsigned char *st = stages + (size_t)(q % nst) * STRIP_STAGE;
                     const int cbase = (part * cpp + cc) * BPC;
 #pragma unroll
                     for (int u = 0; u < BPC; u++) {
@@ -287,13 +235,13 @@ __global__ void __launch_bounds__(NWARP * 32, 1) gemm8_kernel(const GemvParams p
                         if (WDT == JL_Q4) {
                             // bytes [4t, 4t+4) of a block = low nibbles of elements 4t..4t+3 and high nibbles of elements 16+4t..19+4t: the
                             // k-slots of this lane's A fragment registers a0 / a2 (rows g, g+8 -> a0,a2 / a1,a3)
-                            const uint32_t w0 = *(const uint32_t *)(st + g * G8_ROWB + u * 16 + 4 * t), w1 = *(const uint32_t *)(st + (g + 8) * G8_ROWB + u * 16 + 4 * t);
+                            const uint32_t w0 = *(const uint32_t *)(st + g * S::ROWB + u * 16 + 4 * t), w1 = *(const uint32_t *)(st + (g + 8) * S::ROWB + u * 16 + 4 * t);
                             mma_u8s8(c, w0 & 0x0F0F0F0Fu, w1 & 0x0F0F0F0Fu, (w0 >> 4) & 0x0F0F0F0Fu, (w1 >> 4) & 0x0F0F0F0Fu, bl, bh);
                         } else {
-                            const unsigned char *r0p = st + g * G8_ROWB + u * 32 + 4 * t, *r1p = st + (g + 8) * G8_ROWB + u * 32 + 4 * t;
+                            const unsigned char *r0p = st + g * S::ROWB + u * 32 + 4 * t, *r1p = st + (g + 8) * S::ROWB + u * 32 + 4 * t;
                             mma_s8s8(c, *(const uint32_t *)r0p, *(const uint32_t *)r1p, *(const uint32_t *)(r0p + 16), *(const uint32_t *)(r1p + 16), bl, bh);
                         }
-                        const float sw0 = *(const float *)(st + G8_SC_OFF + g * SCS + u * 4), sw1 = *(const float *)(st + G8_SC_OFF + (g + 8) * SCS + u * 4);
+                        const float sw0 = *(const float *)(st + S::SC_OFF + g * SCS + u * 4), sw1 = *(const float *)(st + S::SC_OFF + (g + 8) * SCS + u * 4);
                         // c[0] = (row g, session 2t), c[1] = (row g, 2t+1), c[2] = (row g+8, 2t), c[3] = (row g+8, 2t+1)
                         const uint2 s0 = ass[(2 * t) * sst + b], s1 = ass[(2 * t + 1) * sst + b];
                         const float sa0 = __uint_as_float(s0.x), sa1 = __uint_as_float(s1.x);
@@ -349,7 +297,7 @@ __global__ void __launch_bounds__(NWARP * 32, 1) gemm8_kernel(const GemvParams p
             }
         }
     }
-    g8_wait(0);
+    cp_wait(0);
     if (p.trace) {
         __syncthreads();
         ktrace_end(p.trace);
@@ -361,10 +309,10 @@ static size_t g8_red_bytes(int nwarp) { return (size_t)2 * nwarp * 2 * 128 * 4; 
 static int g8_stages(const GemvParams &p, int nwarp) {
     const size_t act = g8_act_smem(p) + g8_red_bytes(nwarp);
     if (act + 2048 >= G8_SMEM_LIMIT) return 0;
-    int n = (int)((G8_SMEM_LIMIT - 2048 - act) / ((size_t)nwarp * G8_STAGE));
+    int n = (int)((G8_SMEM_LIMIT - 2048 - act) / ((size_t)nwarp * STRIP_STAGE));
     return n > G8_MAX_STAGES ? G8_MAX_STAGES : n;
 }
-static size_t g8_smem(const GemvParams &p, int nwarp) { return g8_act_smem(p) + g8_red_bytes(nwarp) + (size_t)g8_stages(p, nwarp) * nwarp * G8_STAGE; }
+static size_t g8_smem(const GemvParams &p, int nwarp) { return g8_act_smem(p) + g8_red_bytes(nwarp) + (size_t)g8_stages(p, nwarp) * nwarp * STRIP_STAGE; }
 // warps per CTA: 16 while every warp still gets a 3-stage pipeline
 static int g8_warps(const GemvParams &p) { return g8_stages(p, 16) >= 3 ? 16 : 8; }
 // warps of a CTA sharing one strip: the largest of 8, 4, 2, 1 that divides the chunk count of a row

@@ -158,7 +158,6 @@ __global__ void __launch_bounds__(GEMV_THREADS, MINB) gemv_kernel(const GemvPara
 // touched in shared memory and, after a barrier, one thread per output row adds the partials in chunk order
 // (deterministic).  The kernel is kept small on purpose: five different kernels alternate every ~50 us, each starts
 // with a cold instruction cache, and every kilobyte on the prologue path showed up in the timeline (tools/ktrace.py).
-__device__ __forceinline__ int item_owner(int i, int items, int nwarp) { return (int)((((long long)(i + 1)) * nwarp - 1) / items); }
 
 template <int WDT, int EPI, int PRO, int CH, int NBUF, int NT, bool LONG>
 __global__ void __launch_bounds__(NT, 1) gemv_decode_kernel(const GemvParams p, const int) {

@@ -425,6 +425,10 @@ __device__ void stage_q8_pairs(const GemvParams &p, const bool norm, unsigned ch
     __syncthreads();
 }
 
+// LONG rows of the decode GEMV (gemv_decode_kernel and the persistent kernel's phases): the warp that owns item i of a CTA's
+// `items` when they are dealt to `nwarp` warps in order
+__device__ __forceinline__ int item_owner(int i, int items, int nwarp) { return (int)((((long long)(i + 1)) * nwarp - 1) / items); }
+
 // ---- per-chunk math -------------------------------------------------------------------------------
 template <int WDT, bool ACTQ8, int MM, int CH>
 __device__ __forceinline__ void compute_chunk(const WBuf<WDT, CH> &w, float (&acc)[MM], const unsigned char *smem, int blk0,

@@ -133,7 +133,6 @@ __device__ __forceinline__ float ll_load(const int pz, const uint4 *mine, int sr
     return __uint_as_float(v);
 }
 
-__device__ __forceinline__ int item_owner_pd(int i, int items, int nwarp) { return (int)((((long long)(i + 1)) * nwarp - 1) / items); }
 __device__ __forceinline__ unsigned long long pd_pack_arg(float v, int idx) {
     if (!(v == v)) return 0ull; // NaN never wins (AbstractModel.java:465: 'v > maxv' is false)
     uint32_t b = __float_as_uint(v);
@@ -228,11 +227,7 @@ __device__ PD_PHASE_FN void pd_gemv(const int, const int L, const uint32_t tag, 
         }
         const uint8_t *w;
         const float *s;
-#ifdef PD_X_FIXEDW
-        w = CP.lm_w, s = CP.lm_s;
-#else
         ph_weights<PH>(L, seg, w, s);
-#endif
         const size_t blk = (size_t)local * (size_t)nblk;
         wrow = w + blk * WB;
         srow = s + blk;
@@ -269,10 +264,8 @@ __device__ PD_PHASE_FN void pd_gemv(const int, const int L, const uint32_t tag, 
             li++;
         }
     }
-#ifndef PD_X_NOWAIT
     pd_wait(pz, dep_which, dep_target);
     pd_stamp(pz, stamp_idx);
-#endif
     {
         GemvParams p; // only the staging fields; dead after the prologue
         p.a = PH == PH_QKV ? CP.x : (PH == PH_O ? CP.att : (PH == PH_GU ? CP.xb : CP.h));
@@ -327,7 +320,7 @@ __device__ PD_PHASE_FN void pd_gemv(const int, const int L, const uint32_t tag, 
                     const float v = warp_sum(acc[0]);
                     const int rw = cur.r * NW + cur.wr;
                     // slot as in gemv_decode_kernel: the owner's offset when every warp owns an item, else the chunk (one item per warp)
-                    const int slot = items >= NWARP ? warp - item_owner_pd(rw * nchunks, items, NWARP) : cur.c;
+                    const int slot = items >= NWARP ? warp - item_owner(rw * nchunks, items, NWARP) : cur.c;
                     if (lane == 0) parts[rw * maxsplit + slot] = v;
                     acc[0] = 0.0f;
                 }
@@ -345,8 +338,8 @@ __device__ PD_PHASE_FN void pd_gemv(const int, const int L, const uint32_t tag, 
 #pragma unroll
             for (int wr = 0; wr < NW; wr++) {
                 const int rw = o * NW + wr;
-                const int wa = items >= NWARP ? item_owner_pd(rw * nchunks, items, NWARP) : 0;
-                const int ns = items >= NWARP ? item_owner_pd(rw * nchunks + nchunks - 1, items, NWARP) - wa + 1 : nchunks;
+                const int wa = items >= NWARP ? item_owner(rw * nchunks, items, NWARP) : 0;
+                const int ns = items >= NWARP ? item_owner(rw * nchunks + nchunks - 1, items, NWARP) - wa + 1 : nchunks;
                 float t = 0.0f;
                 for (int s = 0; s < ns; s++) t = __fadd_rn(t, parts[rw * maxsplit + s]);
                 sums[wr] = t;
