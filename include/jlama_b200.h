@@ -397,6 +397,34 @@ int jl_model_generate_penalized(jl_model *m, int session, const int32_t *prompt,
 /* The penalty kernel on HOST buffers, for crafted rows: n rows of `vocab` logits at stride ld -> out [n][vocab], the processed rows.
  * pen nullable.  Refused (JL_ERR_INVALID) before any device work as the model calls, and for n < 1. */
 int jl_apply_penalties(jl_ctx *ctx, int n, int vocab, const float *logits, int64_t ld, const jl_penalties *pen, float *out);
+/* ---- constrained decoding: per-row allowed-token masks, this project's rule (DESIGN §3.18) ----------------------------------------
+ * A grammar engine above the model (JSON mode, JSON schema, regex, choices) turns its state into the set A of tokens allowed at the next
+ * position; the calls below apply it.  A is a bitmask of words = (vocab + 31) / 32 uint32 words: token t is allowed when bit t % 32 of
+ * word t / 32 is set; bits at or above vocab are ignored.  allow (HOST [n_allow][words]) holds the call's mask rows and allow_row (HOST
+ * [n], -1 = unconstrained; NULL = no constrained row) gives each row its mask row; rows may share one.  For a constrained row:
+ *   p_t = t in A ? b_t : -inf, b the processed row of the penalties (the raw row without them), so a penalty never brings a banned
+ *   token back;  temperature 0: the arg-max of p, first index on ties;  temperature > 0: the top-k / top-p rule (DESIGN §3.12) on p
+ *   with the row's top_k / top_p (0 / 1 = none), never the reference's prefix-sum rule, which can return a banned token.
+ * Logprobs, logits_out and the KV stay those of the raw logits.  Unconstrained rows get exactly what the _penalized call gives them.
+ * Refused before any device work, leaving the KV as it was: allow_row[i] outside [-1, n_allow), n_allow > 0 with a NULL allow, a
+ * constrained row whose mask allows no token below vocab, everything the _penalized calls refuse (JL_ERR_INVALID); tp_size > 1
+ * (JL_ERR_UNSUPPORTED).  allow_row NULL is the _penalized call, kernel launches included.  The first call with a constrained row
+ * allocates the mask buffers (min(max_sessions, 64) x words uint32, on the device and pinned) and the penalty buffers; they live until
+ * jl_model_free. */
+int jl_model_decode_constrained(jl_model *m, int n, const int32_t *sessions, const int32_t *tokens, const int32_t *positions,
+                                const float *temperatures, const int32_t *top_k, const float *top_p, const float *uniforms,
+                                const int32_t *top_n, const jl_penalties *pen, int n_allow, const uint32_t *allow, const int32_t *allow_row,
+                                int32_t *next_tokens, float *lp_out, int32_t *top_ids_out, float *top_lp_out, float *logits_out);
+int jl_model_sample_multi_constrained(jl_model *m, int n, const int32_t *sessions, const float *temperatures, const int32_t *top_k,
+                                      const float *top_p, const float *uniforms, const int32_t *top_n, const jl_penalties *pen, int n_allow,
+                                      const uint32_t *allow, const int32_t *allow_row, int32_t *tokens_out, float *lp_out,
+                                      int32_t *top_ids_out, float *top_lp_out, float *logits_out);
+/* The selection of the calls above on HOST buffers, for crafted rows: n rows of `vocab` logits at stride ld -> out [n], the tokens.
+ * Unconstrained sampled rows without a filter take the reference's rule, as in the model calls.  Refused (JL_ERR_INVALID) before any
+ * device work as the model calls, and for n < 1 or a vocabulary above 2^23. */
+int jl_select_constrained(jl_ctx *ctx, int n, int vocab, const float *logits, int64_t ld, const float *temperatures, const int32_t *top_k,
+                          const float *top_p, const float *uniforms, const jl_penalties *pen, int n_allow, const uint32_t *allow,
+                          const int32_t *allow_row, int32_t *out);
 /* The mixture-of-experts router kernel on HOST buffers, for crafted rows: n rows of n_experts logits (contiguous) -> probs_out [n][n_experts]
  * (the reference's float softmax: (float)exp((double)(x - max)), a float sum in index order, a divide) and sel_out [n][k], the experts
  * of the replace-the-minimum top-k scan (MoEBlock.java:151-168) in the scan's order.  Refused (JL_ERR_INVALID) before any device work:
@@ -537,6 +565,8 @@ typedef struct jl_sched jl_sched;
 /* submit flags */
 #define JL_SCHED_KEEP_SESSION 1 /* keep the session slot and its KV after the request finishes, for a continuation (the reference's
                                    session header: the next generate() on that UUID starts at kvmem.getCurrentContextPosition(), :533) */
+#define JL_SCHED_CONSTRAINED 2  /* select every token of the request under the allowed-token mask its mask provider gives for it (DESIGN
+                                   §3.18); needs jl_sched_set_mask_provider and a constraint backend */
 /* the four model calls the policy is written against; all return JL_OK or a JL_ERR_* */
 typedef struct {
     int (*reset_session)(void *user, int session);                                                   /* jl_model_reset_session */
@@ -595,6 +625,31 @@ typedef struct {
                                   const float *top_p, const float *uniforms, const int32_t *top_n, const jl_penalties *pen, int32_t *tokens_out,
                                   float *lp_out, int32_t *top_ids_out, float *top_lp_out);
 } jl_sched_penalty_backend;
+/* optional constrained calls (jl_model_decode_constrained / jl_model_sample_multi_constrained without logits) and the vocabulary they
+ * select from, installed with jl_sched_set_constraint_backend.  A decode or first-token call that holds at least one JL_SCHED_CONSTRAINED
+ * request goes through these for all of its rows (the others with allow_row -1; penalties, top_n and top-k / top-p as in the penalty
+ * calls); a call without one is exactly the call it would be without this backend. */
+typedef struct {
+    int (*decode_constrained)(void *user, int n, const int32_t *sessions, const int32_t *tokens, const int32_t *positions,
+                              const float *temperatures, const int32_t *top_k, const float *top_p, const float *uniforms, const int32_t *top_n,
+                              const jl_penalties *pen, int n_allow, const uint32_t *allow, const int32_t *allow_row, int32_t *next_tokens,
+                              float *lp_out, int32_t *top_ids_out, float *top_lp_out);
+    int (*sample_multi_constrained)(void *user, int n, const int32_t *sessions, const float *temperatures, const int32_t *top_k,
+                                    const float *top_p, const float *uniforms, const int32_t *top_n, const jl_penalties *pen, int n_allow,
+                                    const uint32_t *allow, const int32_t *allow_row, int32_t *tokens_out, float *lp_out, int32_t *top_ids_out,
+                                    float *top_lp_out);
+    int vocab; /* the mask width: (vocab + 31) / 32 words */
+} jl_sched_constraint_backend;
+/* The mask provider of JL_SCHED_CONSTRAINED requests: the caller's grammar engine.  Called once before every selection of such a
+ * request -- its first token with n_generated 0, then each decode step with every token the request has generated so far, the one fed
+ * in that step included (for a continuation: this request's tokens only).  It writes the allowed set of the next token into
+ * allow_out [(vocab + 31) / 32] (zeroed before the call) and returns 0.  It runs on the stepping thread without the scheduler's lock
+ * and gets a copy of the tokens: it may call jl_sched_result, jl_sched_cancel and the other request calls, but must not step.  A
+ * non-zero return or a mask that allows no token below vocab fails that request alone (JL_FINISH_ERROR, jl_sched_last_error says
+ * why); the other rows of its call go on.  When the grammar is complete the provider allows only stop tokens, and the request ends
+ * with JL_FINISH_STOP_TOKEN (its first token is not stop-checked, as everywhere). */
+typedef int(jl_sched_mask_fn)(void *user, int64_t request, const int32_t *generated, int n_generated, uint32_t *allow_out); /* a function
+                                                                                                                     type: take it by pointer */
 typedef struct {
     int admitted, prefill_tokens, decode_rows, decode_calls, finished; /* what this step (or run) did */
     int active, queued;                                                 /* afterwards */
@@ -629,6 +684,11 @@ int jl_sched_set_logprob_backend(jl_sched *s, const jl_sched_logprob_backend *lb
 /* install the penalty calls (both set); before the first jl_sched_step only.  jl_sched_create installs the model's
  * jl_model_decode_penalized / jl_model_sample_multi_penalized. */
 int jl_sched_set_penalty_backend(jl_sched *s, const jl_sched_penalty_backend *pb);
+/* install the constrained calls (both set, vocab >= 1); before the first jl_sched_step only.  jl_sched_create installs the model's
+ * jl_model_decode_constrained / jl_model_sample_multi_constrained and its vocab_size. */
+int jl_sched_set_constraint_backend(jl_sched *s, const jl_sched_constraint_backend *cb);
+/* install (fn NULL: remove) the mask provider of JL_SCHED_CONSTRAINED requests, called with `user`; before the first jl_sched_step only */
+int jl_sched_set_mask_provider(jl_sched *s, jl_sched_mask_fn *fn, void *user);
 /* optional fork call (jl_model_kv_fork), installed with jl_sched_set_fork_backend: n completions of one prompt (jl_sched_submit_n).  In the
  * step that forwards the prompt's last chunk, after the forward, one fork(leader session, positions after the prompt, n - 1, sibling
  * sessions) call gives the siblings the prompt's KV and last row; their first tokens then come from the same first-token calls as every
@@ -667,7 +727,8 @@ int jl_sched_request_cached(jl_sched *s, int64_t request);
 int jl_sched_free(jl_sched *s);
 const char *jl_sched_last_error(jl_sched *s);
 /* Queue a request: prompt token ids, at most max_new generated tokens (the first is sampled from the prompt's last row and, like the
- * reference's, not stop-checked), optional stop tokens.  continue_request >= 0: a finished JL_SCHED_KEEP_SESSION request whose session
+ * reference's, not stop-checked), optional stop tokens.  flags: JL_SCHED_KEEP_SESSION, JL_SCHED_CONSTRAINED (refused, -1, without a
+ * mask provider and a constraint backend); every submit call takes them.  continue_request >= 0: a finished JL_SCHED_KEEP_SESSION request whose session
  * this request appends to.  temperature 0 = arg-max; otherwise every token is drawn with the reference's rule (AbstractModel.java:475-489)
  * from a per-request uniform stream seeded with `seed` (the reference draws ThreadLocalRandom.nextFloat(), :576,:594): the k-th token of
  * a request uses its k-th draw however the steps were batched, so (seed, prompt) reproduces.  Returns the request id (> 0) or -1.

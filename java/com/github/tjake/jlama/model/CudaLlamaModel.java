@@ -90,6 +90,14 @@ public final class CudaLlamaModel implements AutoCloseable {
     private static final MethodHandle jl_model_decode_penalized =
         h("jl_model_decode_penalized", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS,
                                                              ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS));
+    private static final MethodHandle jl_model_decode_constrained =
+        h("jl_model_decode_constrained", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS,
+                                                               ADDRESS, ADDRESS, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS,
+                                                               ADDRESS, ADDRESS));
+    private static final MethodHandle jl_model_sample_multi_constrained =
+        h("jl_model_sample_multi_constrained", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS,
+                                                                     ADDRESS, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS,
+                                                                     ADDRESS, ADDRESS));
     private static final MethodHandle jl_model_generate_penalized =
         h("jl_model_generate_penalized", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, JAVA_INT, JAVA_INT, JAVA_FLOAT, JAVA_INT,
                                                                JAVA_FLOAT, ADDRESS, JAVA_INT, JAVA_FLOAT, JAVA_FLOAT, JAVA_FLOAT, JAVA_INT, ADDRESS,
@@ -372,6 +380,75 @@ public final class CudaLlamaModel implements AutoCloseable {
             check((int) jl_model_decode_penalized.invokeExact(model, n, s, t, p, tt, k, tp, u, tn, pen, nxt, lp, ids, tlp, MemorySegment.NULL), ctx);
             logprobs[0] = TokenLogprobs.of(lp, ids, tlp, n);
             return nxt.toArray(JAVA_INT);
+        } catch (RuntimeException | Error e) { throw e; } catch (Throwable t) { throw new RuntimeException(t); }
+    }
+
+    /** the vocabulary of the model: the width of its allowed-token masks is (vocab + 31) / 32 words */
+    public int vocabularySize() {
+        return c.vocabularySize;
+    }
+
+    /**
+     * Allowed-token masks of one call (DESIGN §3.18): a null row is unconstrained, otherwise token t is allowed where allowed[i][t].
+     * Returns {allow [n_allow][words], allow_row [n]}; n_allow = the constrained rows.
+     */
+    static MemorySegment[] masks(Arena a, boolean[][] allowed, int vocab) {
+        int words = (vocab + 31) / 32, nAllow = 0;
+        for (boolean[] r : allowed) if (r != null) nAllow++;
+        MemorySegment allow = a.allocate(JAVA_INT, Math.max(1, (long) nAllow * words)), rows = a.allocate(JAVA_INT, allowed.length);
+        int k = 0;
+        for (int i = 0; i < allowed.length; i++) {
+            rows.setAtIndex(JAVA_INT, i, allowed[i] == null ? -1 : k);
+            if (allowed[i] == null) continue;
+            for (int t = 0; t < vocab; t++)
+                if (allowed[i][t]) {
+                    long w = (long) k * words + t / 32;
+                    allow.setAtIndex(JAVA_INT, w, allow.getAtIndex(JAVA_INT, w) | (1 << (t % 32)));
+                }
+            k++;
+        }
+        return new MemorySegment[] {allow, rows, MemorySegment.ofArray(new int[] {nAllow})};
+    }
+
+    /**
+     * decode() with penalties and allowed-token masks (a grammar engine's masks for JSON mode, a JSON schema, a regex or a choice; DESIGN
+     * §3.18): each constrained row is selected from its processed logits with every token outside its allowed set at -inf, greedy rows
+     * by the arg-max, sampled rows by the top-k / top-p rule.  Null mask rows are exactly what the penalties-only decode() gives them.
+     */
+    public int[] decode(int[] sessions, int[] tokens, int[] positions, float[] temperatures, int[] topK, float[] topP, float[] uniforms, int[] topN,
+                        Penalties[] penalties, boolean[][] allowed, TokenLogprobs[] logprobs) {
+        try (Arena a = Arena.ofConfined()) {
+            int n = tokens.length;
+            MemorySegment s = a.allocateFrom(JAVA_INT, sessions), t = a.allocateFrom(JAVA_INT, tokens), p = a.allocateFrom(JAVA_INT, positions);
+            MemorySegment tt = a.allocateFrom(JAVA_FLOAT, temperatures), k = a.allocateFrom(JAVA_INT, topK), tp = a.allocateFrom(JAVA_FLOAT, topP);
+            MemorySegment u = a.allocateFrom(JAVA_FLOAT, uniforms), tn = a.allocateFrom(JAVA_INT, topN), nxt = a.allocate(JAVA_INT, n);
+            MemorySegment lp = a.allocate(JAVA_FLOAT, n), ids = a.allocate(JAVA_INT, (long) n * MAX_LOGPROBS), tlp = a.allocate(JAVA_FLOAT, (long) n * MAX_LOGPROBS);
+            MemorySegment pen = penalties(a, penalties);
+            MemorySegment[] m = masks(a, allowed, c.vocabularySize);
+            int nAllow = m[2].getAtIndex(JAVA_INT, 0);
+            check((int) jl_model_decode_constrained.invokeExact(model, n, s, t, p, tt, k, tp, u, tn, pen, nAllow, m[0], m[1], nxt, lp, ids, tlp,
+                                                                MemorySegment.NULL), ctx);
+            logprobs[0] = TokenLogprobs.of(lp, ids, tlp, n);
+            return nxt.toArray(JAVA_INT);
+        } catch (RuntimeException | Error e) { throw e; } catch (Throwable t) { throw new RuntimeException(t); }
+    }
+
+    /** The first tokens of n prefilled sessions under penalties and allowed-token masks, as decode() above.  Fills `logprobs`. */
+    public int[] sampleMulti(int[] sessions, float[] temperatures, int[] topK, float[] topP, float[] uniforms, int[] topN, Penalties[] penalties,
+                             boolean[][] allowed, TokenLogprobs[] logprobs) {
+        try (Arena a = Arena.ofConfined()) {
+            int n = sessions.length;
+            MemorySegment s = a.allocateFrom(JAVA_INT, sessions), tt = a.allocateFrom(JAVA_FLOAT, temperatures), k = a.allocateFrom(JAVA_INT, topK);
+            MemorySegment tp = a.allocateFrom(JAVA_FLOAT, topP), u = a.allocateFrom(JAVA_FLOAT, uniforms), tn = a.allocateFrom(JAVA_INT, topN);
+            MemorySegment out = a.allocate(JAVA_INT, n), lp = a.allocate(JAVA_FLOAT, n), ids = a.allocate(JAVA_INT, (long) n * MAX_LOGPROBS);
+            MemorySegment tlp = a.allocate(JAVA_FLOAT, (long) n * MAX_LOGPROBS);
+            MemorySegment pen = penalties(a, penalties);
+            MemorySegment[] m = masks(a, allowed, c.vocabularySize);
+            int nAllow = m[2].getAtIndex(JAVA_INT, 0);
+            check((int) jl_model_sample_multi_constrained.invokeExact(model, n, s, tt, k, tp, u, tn, pen, nAllow, m[0], m[1], out, lp, ids, tlp,
+                                                                      MemorySegment.NULL), ctx);
+            logprobs[0] = TokenLogprobs.of(lp, ids, tlp, n);
+            return out.toArray(JAVA_INT);
         } catch (RuntimeException | Error e) { throw e; } catch (Throwable t) { throw new RuntimeException(t); }
     }
 

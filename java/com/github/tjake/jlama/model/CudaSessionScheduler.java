@@ -17,6 +17,8 @@ package com.github.tjake.jlama.model;
 
 import java.lang.foreign.*;
 import java.lang.invoke.MethodHandle;
+import java.lang.invoke.MethodHandles;
+import java.lang.invoke.MethodType;
 import java.util.Map;
 import java.util.UUID;
 import java.util.concurrent.ConcurrentHashMap;
@@ -27,7 +29,7 @@ import static java.lang.foreign.ValueLayout.*;
 public final class CudaSessionScheduler implements AutoCloseable {
     public static final int QUEUED = 0, PREFILL = 1, DECODING = 2, FINISHED = 3, FAILED = 4;          // JL_SCHED_*
     public static final int MAX_TOKENS = 1, STOP_TOKEN = 2, CANCELLED = 3, ERROR = 4;                    // JL_FINISH_* (Generator.FinishReason)
-    private static final int KEEP_SESSION = 1;
+    private static final int KEEP_SESSION = 1, CONSTRAINED = 2;                                      // JL_SCHED_* submit flags
 
     private static final Linker LINKER = Linker.nativeLinker();
     private static final SymbolLookup LIB = SymbolLookup.loaderLookup().or(LINKER.defaultLookup());
@@ -54,6 +56,8 @@ public final class CudaSessionScheduler implements AutoCloseable {
     private static final MethodHandle jl_sched_release = h("jl_sched_release", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_LONG));
     private static final MethodHandle jl_sched_set_prefix_cache =
         h("jl_sched_set_prefix_cache", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, JAVA_INT));
+    private static final MethodHandle jl_sched_set_mask_provider =
+        h("jl_sched_set_mask_provider", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, ADDRESS));
     private static final MethodHandle jl_sched_prefix_stats = h("jl_sched_prefix_stats", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS));
 
     private final Arena arena = Arena.ofShared();
@@ -69,11 +73,45 @@ public final class CudaSessionScheduler implements AutoCloseable {
     }
 
     /**
+     * The grammar engine of constrained requests (JSON mode, a JSON schema, tool-call arguments, a regex; DESIGN §3.18): the allowed set
+     * of the next token of `request` after the tokens it has `generated` (none for its first token), indexed by token id.  Called once
+     * before every selection of a constrained request, on the stepping thread; it must not block on generate() of the same scheduler.
+     * When the grammar is complete it allows only the request's stop tokens.  Throwing fails that request alone.
+     */
+    @FunctionalInterface
+    public interface MaskProvider {
+        boolean[] allowed(long request, int[] generated);
+    }
+
+    private MaskProvider maskProvider;
+    private int vocab;
+
+    /** jl_sched_mask_fn upcall: the provider's set -> allow_out [(vocab + 31) / 32] (zeroed by the scheduler); non-zero on failure */
+    private int mask(MemorySegment user, long request, MemorySegment generated, int n, MemorySegment allowOut) {
+        try {
+            int[] gen = n == 0 ? new int[0] : generated.reinterpret(4L * n).toArray(JAVA_INT);
+            boolean[] a = maskProvider.allowed(request, gen);
+            MemorySegment out = allowOut.reinterpret(4L * ((vocab + 31) / 32));
+            for (int t = 0; t < vocab && t < a.length; t++)
+                if (a[t]) out.setAtIndex(JAVA_INT, t / 32, out.getAtIndex(JAVA_INT, t / 32) | (1 << (t % 32)));
+            return 0;
+        } catch (Throwable t) {
+            return 1; // an exception must not unwind through the native caller
+        }
+    }
+
+
+    /**
      * prefixCachePages > 0: requests without a session reuse the KV pages of earlier prompts that share a whole-page prefix with theirs,
      * the cache holding at most that many pages no session holds (DESIGN §3.17).  A stateless chat client that resends its whole
      * conversation then forwards only the new turn.
      */
     public CudaSessionScheduler(CudaLlamaModel model, int maxActive, int prefillTokensPerStep, int prefixCachePages) {
+        this(model, maxActive, prefillTokensPerStep, prefixCachePages, null);
+    }
+
+    /** A scheduler whose constrained requests (generate(..., constrained = true, ...)) take their allowed sets from maskProvider (nullable). */
+    public CudaSessionScheduler(CudaLlamaModel model, int maxActive, int prefillTokensPerStep, int prefixCachePages, MaskProvider maskProvider) {
         try {
             MemorySegment out = arena.allocate(ADDRESS);
             int rc = (int) jl_sched_create.invokeExact(model.handle(), maxActive, prefillTokensPerStep, out);
@@ -84,6 +122,18 @@ public final class CudaSessionScheduler implements AutoCloseable {
                 if (rc != 0) {
                     int ignored = (int) jl_sched_free.invokeExact(sched);
                     throw new IllegalStateException("jl_sched_set_prefix_cache: " + rc);
+                }
+            }
+            if (maskProvider != null) { // before the stepping thread's first step
+                this.maskProvider = maskProvider;
+                this.vocab = model.vocabularySize();
+                MethodHandle up = MethodHandles.lookup().findVirtual(CudaSessionScheduler.class, "mask",
+                        MethodType.methodType(int.class, MemorySegment.class, long.class, MemorySegment.class, int.class, MemorySegment.class)).bindTo(this);
+                MemorySegment stub = LINKER.upcallStub(up, FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_LONG, ADDRESS, JAVA_INT, ADDRESS), arena);
+                rc = (int) jl_sched_set_mask_provider.invokeExact(sched, stub, MemorySegment.NULL);
+                if (rc != 0) {
+                    int ignored = (int) jl_sched_free.invokeExact(sched);
+                    throw new IllegalStateException("jl_sched_set_mask_provider: " + rc);
                 }
             }
         } catch (RuntimeException | Error e) { throw e; } catch (Throwable t) { throw new RuntimeException(t); }
@@ -198,6 +248,15 @@ public final class CudaSessionScheduler implements AutoCloseable {
      */
     public int generate(UUID session, int[] promptTokens, float temperature, int topK, float topP, int maxNew, int[] eosTokens, boolean keepSession,
                         int logprobs, CudaLlamaModel.Penalties penalties, TokenLogprobConsumer onToken) {
+        return generate(session, promptTokens, temperature, topK, topP, maxNew, eosTokens, keepSession, false, logprobs, penalties, onToken);
+    }
+
+    /**
+     * generate() under a grammar (DESIGN §3.18): with constrained = true every token is selected under the allowed set the scheduler's
+     * MaskProvider gives for it, after the penalties.  A request whose provider throws or allows nothing ends with ERROR.
+     */
+    public int generate(UUID session, int[] promptTokens, float temperature, int topK, float topP, int maxNew, int[] eosTokens, boolean keepSession,
+                        boolean constrained, int logprobs, CudaLlamaModel.Penalties penalties, TokenLogprobConsumer onToken) {
         final int W = CudaLlamaModel.MAX_LOGPROBS;
         try (Arena a = Arena.ofConfined()) {
             MemorySegment pr = a.allocateFrom(JAVA_INT, promptTokens);
@@ -205,7 +264,8 @@ public final class CudaSessionScheduler implements AutoCloseable {
             MemorySegment bi = a.allocateFrom(JAVA_INT, penalties.biasIds()), bv = a.allocateFrom(JAVA_FLOAT, penalties.biasValues());
             Long parent = kept.remove(session);
             long id = (long) jl_sched_submit_penalized.invokeExact(sched, pr, promptTokens.length, maxNew, eos, eosTokens.length,
-                                                                    keepSession ? KEEP_SESSION : 0, parent == null ? -1L : (long) parent,
+                                                                    (keepSession ? KEEP_SESSION : 0) | (constrained ? CONSTRAINED : 0),
+                                                                    parent == null ? -1L : (long) parent,
                                                                     temperature, topK, topP, java.util.concurrent.ThreadLocalRandom.current().nextLong(),
                                                                     logprobs, penalties.presence(), penalties.frequency(), penalties.repetition(),
                                                                     penalties.biasIds().length, bi, bv);

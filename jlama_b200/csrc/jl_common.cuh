@@ -240,6 +240,7 @@ struct PenaltyRow {
     int32_t on;                    // 0: the row is copied unchanged
     int32_t hist0, prompt1, hist1; // history [hist0, hist1), of which [hist0, prompt1) are prompt tokens
     int32_t bias0, bias1;          // bias entries [bias0, bias1)
+    int32_t mask;                  // allowed-token mask row of the call (DESIGN §3.18), -1 = unconstrained
 };
 struct PenaltyPlan {
     int n_on = 0;        // penalised rows
@@ -252,8 +253,19 @@ int jl_penalty_check(jl_ctx *ctx, const char *who, int n, int vocab, const jl_pe
 void jl_penalty_pack(const jl_penalties *pen, int n, const PenaltyPlan &plan, void *tab);
 // Two launches for all n rows: the histories and bias lists of the penalised rows are marked in cnt / bias (DEVICE [n][vocab] each; cnt
 // zero before the first launch, and each launch leaves it zero), then every row of logits (read-only, stride ld) -> out [n][vocab].
+// mask (DEVICE [rows][(vocab + 31) / 32], nullable): the allowed-token mask rows the table's PenaltyRow::mask index; a row's banned
+// tokens become -inf after its penalties.  With a mask and no penalised row the mark launch is skipped.
 int jl_launch_penalties(jl_ctx *ctx, cudaStream_t s, const float *logits, int64_t ld, int vocab, int n, const void *tab,
-                        const PenaltyPlan &plan, unsigned *cnt, float *bias, float *out);
+                        const PenaltyPlan &plan, unsigned *cnt, float *bias, const uint32_t *mask, float *out);
+// Allowed-token masks of the *_constrained calls (DESIGN §3.18): allow (HOST [n_allow][(vocab + 31) / 32]) and allow_row (HOST [n],
+// nullable = no constrained row; -1 = unconstrained).  Refused (JL_ERR_INVALID with the error set) before any device work: n_allow < 0,
+// n_allow > 0 with a NULL allow, allow_row[i] outside [-1, n_allow), a constrained row whose mask allows no token below vocab.
+// *n_on = the constrained rows.
+int jl_constraint_check(jl_ctx *ctx, const char *who, int n, int vocab, int n_allow, const uint32_t *allow, const int32_t *allow_row,
+                        int *n_on);
+// the mask rows the constrained rows of a checked call use -> dst (HOST, at most n rows of (vocab + 31) / 32 words, each used row
+// once), and PenaltyRow::mask of the packed table `tab` pointed at them.  Returns the rows written.
+int jl_constraint_pack(int n, int vocab, int n_allow, const uint32_t *allow, const int32_t *allow_row, void *tab, uint32_t *dst);
 // KV page copies (jl_kv_copy.cu; DESIGN §3.15): entry e makes page dst a copy of page src in positions [0, rows) of every layer's K and V
 // block, zeros in the others.  One launch for the n entries of tab (DEVICE); pages are [layers][2][ctx_per_page rows of row_bytes].
 struct KvCopy {

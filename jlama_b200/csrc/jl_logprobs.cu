@@ -210,7 +210,7 @@ int jl_launch_logprobs(jl_ctx *ctx, cudaStream_t st, const float *logits, int64_
 
 void jl_logprobs_unpack(const LogprobOut *o, const int32_t *top_n, int n, float *lp_out, int32_t *top_ids_out, float *top_lp_out) {
     for (int i = 0; i < n; i++) {
-        const bool on = top_n[i] >= 0;
+        const bool on = top_n && top_n[i] >= 0; // top_n NULL: every row without logprobs
         if (lp_out) lp_out[i] = on ? o[i].lp : NAN;
         for (int r = 0; r < JL_MAX_LOGPROBS; r++) {
             const bool slot = on && r < top_n[i];

@@ -90,6 +90,9 @@ struct jl_model {
     unsigned *pen_cnt = nullptr;
     void *d_pen_tab = nullptr, *h_pen_tab = nullptr;
     size_t pen_tab_cap = 0;
+    // allowed-token masks (DESIGN §3.18), allocated by the first call with a constrained row: min(max_sessions, JL_MAX_DECODE_ROWS) rows
+    // of (vocab + 31) / 32 words on the device and in pinned staging
+    uint32_t *d_mask = nullptr, *h_mask = nullptr;
     int hist_cap = 0;
     // graphs keyed by (n, splits, resident)
     std::map<long long, cudaGraphExec_t> graphs;
@@ -687,13 +690,13 @@ extern "C" int64_t jl_model_weight_bytes(jl_model *m) { return m ? m->weight_byt
 int jl_model_num_experts(jl_model *m) { return m ? m->n_exp : 0; } // jl_model_load_safetensors
 
 // limits the session scheduler (jl_sched.cu) plans against: {max_sessions, reserved context, max_batch, rows per decode call,
-// ctx_per_page}
-void jl_model_limits(jl_model *m, int out[5]) {
-    out[0] = out[1] = out[2] = out[3] = out[4] = 0;
+// ctx_per_page, vocab_size}
+void jl_model_limits(jl_model *m, int out[6]) {
+    out[0] = out[1] = out[2] = out[3] = out[4] = out[5] = 0;
     if (!m || !m->finalized) return;
     out[0] = m->cfg.max_sessions, out[1] = m->max_context, out[2] = m->cfg.max_batch;
     out[3] = m->cfg.max_sessions < JL_MAX_DECODE_ROWS ? m->cfg.max_sessions : JL_MAX_DECODE_ROWS;
-    out[4] = m->kv.ctx_per_page;
+    out[4] = m->kv.ctx_per_page, out[5] = m->cfg.vocab_size;
 }
 
 // The timeline buffer was replaced (jl_debug_ktrace): drop every captured decode graph, they are re-captured on demand.
@@ -734,12 +737,13 @@ extern "C" int jl_model_free(jl_model *m) {
     void *bufs[] = {m->d_copy_tab,m->ln, m->hbuf2, m->abf, m->rope, m->page_table_dev, m->x, m->xb, m->q, m->k, m->v, m->att, m->hbuf, m->partial, m->logits,
                     m->last_hidden, m->attn_ws, m->d_tokens, m->d_positions, m->d_sessions, m->d_next, m->d_hist, m->d_counter,
                     m->argmax_scratch, m->fda_done, m->moe_wtab, m->moe_stab, m->moe_logits, m->moe_sel, m->pd_sync, m->pd_slots, m->pd_att_done, m->pd_trace, m->ll_o, m->ll_d, m->ll_a, m->wide_act, m->wide_part, m->wide_cnt, m->d_pa_tab, m->d_rows, m->topkp_ex, m->d_topkp,
-                    m->score_logits, m->pen_out, m->pen_bias, m->pen_cnt, m->d_pen_tab};
+                    m->score_logits, m->pen_out, m->pen_bias, m->pen_cnt, m->d_pen_tab, m->d_mask};
     for (void *p : bufs)
         if (p) cudaFree(p);
     lp_free(m->lp);
     lp_free(m->lp_score);
     if (m->h_pen_tab) cudaFreeHost(m->h_pen_tab);
+    if (m->h_mask) cudaFreeHost(m->h_mask);
     if (m->h_pinned) cudaFreeHost(m->h_pinned);
     if (m->h_topkp) cudaFreeHost(m->h_topkp);
     if (m->ev_begin) cudaEventDestroy(m->ev_begin);
@@ -1681,23 +1685,73 @@ static int penalty_alloc(jl_model *m, size_t bytes) {
     return JL_OK;
 }
 
-// after the logits_out copy: m->logits -> the processed rows m->pen_out (two launches), then the arg-max of every row again on those
-// (the greedy tokens of the decode graphs and the persistent kernel were taken on the raw rows).  The table rides the stream.
-static int penalty_rows(jl_model *m, int n, const PenaltyArgs &a) {
+// Allowed-token masks of one call (the *_constrained entry points; DESIGN §3.18): allow_row nullable; a call without a constrained row
+// runs exactly as the matching _penalized call.
+struct ConstraintArgs {
+    int n_allow = 0;
+    const uint32_t *allow = nullptr;   // HOST [n_allow][words]
+    const int32_t *allow_row = nullptr; // HOST [n], -1 = unconstrained
+    int n_on = 0;                       // constrained rows
+};
+
+// after topkp_check: a constrained row with temperature > 0 is drawn by the top-k / top-p kernel (the integer rule gives a banned
+// token weight 0 and never draws one), whatever its filter
+static int constraint_check(jl_model *m, const char *who, int n, const float *temperatures, const float *uniforms, TopkpArgs &f,
+                            ConstraintArgs &a) {
+    if (!a.allow_row) return JL_OK;
+    jl_ctx *ctx = m->ctx;
+    if (m->cfg.tp_size > 1) return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "%s: constrained rows under tensor parallelism", who);
+    M_CHECK(jl_constraint_check(ctx, who, n, m->cfg.vocab_size, a.n_allow, a.allow, a.allow_row, &a.n_on));
+    for (int i = 0; i < n; i++) {
+        if (a.allow_row[i] < 0 || !temperatures || !(temperatures[i] > 0.0f) || f.filtered[(size_t)i]) continue;
+        if (!(uniforms[i] >= 0.0f && uniforms[i] <= 1.0f))
+            return jl_set_error(ctx, JL_ERR_INVALID, "%s: row %d: uniform %g (in [0, 1])", who, i, (double)uniforms[i]);
+        if (m->cfg.vocab_size > JL_TOPKP_MAX_VOCAB)
+            return jl_set_error(ctx, JL_ERR_INVALID, "%s: vocabulary of %d above %d", who, m->cfg.vocab_size, JL_TOPKP_MAX_VOCAB);
+        f.filtered[(size_t)i] = 1, f.n_filtered++;
+    }
+    return JL_OK;
+}
+
+// the mask buffers for a call with a constrained row (model lock held)
+static int constraint_alloc(jl_model *m) {
+    if (m->d_mask) return JL_OK;
+    jl_ctx *ctx = m->ctx;
+    const int S = m->cfg.max_sessions, rows = S < JL_MAX_DECODE_ROWS ? S : JL_MAX_DECODE_ROWS;
+    const size_t bytes = (size_t)rows * ((m->cfg.vocab_size + 31) / 32) * 4;
+    M_CHECK(dev_alloc(ctx, (void **)&m->d_mask, bytes));
+    JL_CUDA_CHECK(ctx, cudaMallocHost((void **)&m->h_mask, bytes));
+    return JL_OK;
+}
+
+// the table of a call's processed rows: the penalties' own, or one unpenalised PenaltyRow per row for a call with masks only
+static size_t processed_tab_bytes(int n, const PenaltyArgs &a) { return a.pen ? a.plan.bytes : (size_t)n * sizeof(PenaltyRow); }
+
+// after the logits_out copy: m->logits -> the processed rows m->pen_out (penalties, then masks; two launches, one without a penalised
+// row), then the arg-max of every row again on those (the greedy tokens of the decode graphs and the persistent kernel were taken on
+// the raw rows).  The table and the mask rows ride the stream, one copy each.
+static int penalty_rows(jl_model *m, int n, const PenaltyArgs &a, const ConstraintArgs &c) {
     jl_ctx *ctx = m->ctx;
     const int V = m->cfg.vocab_size;
-    jl_penalty_pack(a.pen, n, a.plan, m->h_pen_tab);
-    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(m->d_pen_tab, m->h_pen_tab, a.plan.bytes, cudaMemcpyHostToDevice, m->stream));
-    M_CHECK(jl_launch_penalties(ctx, m->stream, m->logits, V, V, n, m->d_pen_tab, a.plan, m->pen_cnt, m->pen_bias, m->pen_out));
+    const jl_penalties none = {};
+    jl_penalty_pack(a.pen ? a.pen : &none, n, a.plan, m->h_pen_tab);
+    const uint32_t *mask = nullptr;
+    if (c.n_on > 0) {
+        const int rows = jl_constraint_pack(n, V, c.n_allow, c.allow, c.allow_row, m->h_pen_tab, m->h_mask);
+        JL_CUDA_CHECK(ctx, cudaMemcpyAsync(m->d_mask, m->h_mask, (size_t)rows * ((V + 31) / 32) * 4, cudaMemcpyHostToDevice, m->stream));
+        mask = m->d_mask;
+    }
+    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(m->d_pen_tab, m->h_pen_tab, processed_tab_bytes(n, a), cudaMemcpyHostToDevice, m->stream));
+    M_CHECK(jl_launch_penalties(ctx, m->stream, m->logits, V, V, n, m->d_pen_tab, a.plan, m->pen_cnt, m->pen_bias, mask, m->pen_out));
     return jl_launch_argmax(ctx, m->stream, m->pen_out, n, V, V, m->d_next, m->argmax_scratch);
 }
 
-// everything after the logits of one call: penalties, top-k / top-p rows, reference-rule rows, logprobs (of the raw logits)
+// everything after the logits of one call: penalties and masks, top-k / top-p rows, reference-rule rows, logprobs (of the raw logits)
 static int select_rows(jl_model *m, int n, const float *temperatures, const float *uniforms, bool sampled, const TopkpArgs &f, int lp_on,
-                       const PenaltyArgs &pa) {
+                       const PenaltyArgs &pa, const ConstraintArgs &ca) {
     float *src = m->logits;
-    if (pa.plan.n_on > 0) {
-        M_CHECK(penalty_rows(m, n, pa));
+    if (pa.plan.n_on > 0 || ca.n_on > 0) {
+        M_CHECK(penalty_rows(m, n, pa, ca));
         src = m->pen_out;
     }
     M_CHECK(sample_filtered_rows(m, n, temperatures, uniforms, f, src));
@@ -1748,7 +1802,7 @@ static void logprob_unpack(jl_model *m, int n, const LogprobArgs &a) {
 // when `f` filters it.  `lp`: logprobs of the chosen tokens.  `pa`: penalties; the selection of every row then reads its processed row.
 static int decode_impl(jl_model *m, int n, const int32_t *sessions, const int32_t *tokens, const int32_t *positions,
                        const float *temperatures, const float *uniforms, int32_t *next_tokens, float *logits_out, TopkpArgs &&f = TopkpArgs(),
-                       LogprobArgs lp = LogprobArgs(), PenaltyArgs pa = PenaltyArgs()) {
+                       LogprobArgs lp = LogprobArgs(), PenaltyArgs pa = PenaltyArgs(), ConstraintArgs ca = ConstraintArgs()) {
     if (!m || !m->finalized || n <= 0 || n > m->cfg.max_sessions || n > JL_MAX_DECODE_ROWS || !sessions || !tokens || !positions ||
         !next_tokens)
         return m ? jl_set_error(m->ctx, JL_ERR_INVALID, "decode: bad arguments (n=%d, max %d)", n, JL_MAX_DECODE_ROWS) : JL_ERR_INVALID;
@@ -1758,10 +1812,12 @@ static int decode_impl(jl_model *m, int n, const int32_t *sessions, const int32_
     M_CHECK(topkp_check(m, "decode", n, temperatures, uniforms, f));
     M_CHECK(logprobs_check(m, "decode", n, lp));
     M_CHECK(penalty_check(m, "decode", n, pa));
+    M_CHECK(constraint_check(m, "decode", n, temperatures, uniforms, f, ca));
     std::lock_guard<std::recursive_mutex> model_lock(m->mu);
     jl_ctx *ctx = m->ctx;
     JL_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
-    if (pa.plan.n_on > 0) M_CHECK(penalty_alloc(m, pa.plan.bytes));
+    if (pa.plan.n_on > 0 || ca.n_on > 0) M_CHECK(penalty_alloc(m, processed_tab_bytes(n, pa)));
+    if (ca.n_on > 0) M_CHECK(constraint_alloc(m));
     int max_pos = 0;
     for (int i = 0; i < n; i++) {
         if (sessions[i] < 0 || sessions[i] >= m->cfg.max_sessions || positions[i] < 0)
@@ -1773,10 +1829,10 @@ static int decode_impl(jl_model *m, int n, const int32_t *sessions, const int32_
     }
     JL_CUDA_CHECK(ctx, cudaEventRecord(m->ev_begin, m->stream));
     M_CHECK(stage_rows(m, n, tokens, positions, sessions));
-    M_CHECK(run_decode(m, n, max_pos, false, logits_out != nullptr || sampled || pa.plan.n_on > 0));
+    M_CHECK(run_decode(m, n, max_pos, false, logits_out != nullptr || sampled || pa.plan.n_on > 0 || ca.n_on > 0));
     if (logits_out) // before the sampling kernels turn the sampled rows into exponentials in place
         JL_CUDA_CHECK(ctx, cudaMemcpyAsync(logits_out, m->logits, (size_t)n * m->cfg.vocab_size * 4, cudaMemcpyDeviceToHost, m->stream));
-    M_CHECK(select_rows(m, n, temperatures, uniforms, sampled, f, lp.n_on, pa));
+    M_CHECK(select_rows(m, n, temperatures, uniforms, sampled, f, lp.n_on, pa, ca));
     M_CHECK(logprob_rows(m, n, lp));
     JL_CUDA_CHECK(ctx, cudaMemcpyAsync(pinned_next(m), m->d_next, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
     JL_CUDA_CHECK(ctx, cudaEventRecord(m->ev_end, m->stream));
@@ -1794,18 +1850,19 @@ static int decode_impl(jl_model *m, int n, const int32_t *sessions, const int32_
 // launch and share one lm_head pass (sample_rows' wide mode: one weight pass for 9..64 rows).  logits_out gets the raw logits.
 static int sample_sessions(jl_model *m, int n, const int32_t *sessions, const float *temperatures, const float *uniforms,
                            int32_t *tokens_out, float *logits_out, const TopkpArgs &f = TopkpArgs(), const LogprobArgs &lp = LogprobArgs(),
-                           const PenaltyArgs &pa = PenaltyArgs()) {
+                           const PenaltyArgs &pa = PenaltyArgs(), const ConstraintArgs &ca = ConstraintArgs()) {
     std::lock_guard<std::recursive_mutex> model_lock(m->mu);
     jl_ctx *ctx = m->ctx;
     JL_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
-    if (pa.plan.n_on > 0) M_CHECK(penalty_alloc(m, pa.plan.bytes));
+    if (pa.plan.n_on > 0 || ca.n_on > 0) M_CHECK(penalty_alloc(m, processed_tab_bytes(n, pa)));
+    if (ca.n_on > 0) M_CHECK(constraint_alloc(m));
     memcpy(pinned_rows(m), sessions, (size_t)n * 4);
     JL_CUDA_CHECK(ctx, cudaMemcpyAsync(m->d_rows, pinned_rows(m), (size_t)n * 4, cudaMemcpyHostToDevice, m->stream));
     M_CHECK(copy_rows(m, m->xb, nullptr, m->last_hidden, m->d_rows, n));
     M_CHECK(sample_rows(m, m->xb, n));
     if (logits_out) // before the sampled rows are exponentiated in place
         JL_CUDA_CHECK(ctx, cudaMemcpyAsync(logits_out, m->logits, (size_t)n * m->cfg.vocab_size * 4, cudaMemcpyDeviceToHost, m->stream));
-    M_CHECK(select_rows(m, n, temperatures, uniforms, true, f, lp.n_on, pa));
+    M_CHECK(select_rows(m, n, temperatures, uniforms, true, f, lp.n_on, pa, ca));
     M_CHECK(logprob_rows(m, n, lp));
     JL_CUDA_CHECK(ctx, cudaMemcpyAsync(pinned_next(m), m->d_next, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
     JL_CUDA_CHECK(ctx, cudaStreamSynchronize(m->stream));
@@ -1823,7 +1880,7 @@ extern "C" int jl_model_sample(jl_model *m, int session, float temperature, floa
 
 static int sample_multi_impl(jl_model *m, int n, const int32_t *sessions, const float *temperatures, const float *uniforms,
                              int32_t *tokens_out, float *logits_out, TopkpArgs &&f = TopkpArgs(), LogprobArgs lp = LogprobArgs(),
-                             PenaltyArgs pa = PenaltyArgs()) {
+                             PenaltyArgs pa = PenaltyArgs(), ConstraintArgs ca = ConstraintArgs()) {
     if (!m || !m->finalized) return JL_ERR_INVALID;
     jl_ctx *ctx = m->ctx;
     const int S = m->cfg.max_sessions, cap = S < JL_MAX_DECODE_ROWS ? S : JL_MAX_DECODE_ROWS;
@@ -1841,7 +1898,8 @@ static int sample_multi_impl(jl_model *m, int n, const int32_t *sessions, const 
     M_CHECK(topkp_check(m, "sample_multi", n, temperatures, uniforms, f));
     M_CHECK(logprobs_check(m, "sample_multi", n, lp));
     M_CHECK(penalty_check(m, "sample_multi", n, pa));
-    return sample_sessions(m, n, sessions, temperatures, uniforms, tokens_out, logits_out, f, lp, pa);
+    M_CHECK(constraint_check(m, "sample_multi", n, temperatures, uniforms, f, ca));
+    return sample_sessions(m, n, sessions, temperatures, uniforms, tokens_out, logits_out, f, lp, pa, ca);
 }
 
 extern "C" int jl_model_sample_multi(jl_model *m, int n, const int32_t *sessions, const float *temperatures, const float *uniforms,
@@ -1906,6 +1964,109 @@ extern "C" int jl_model_decode_penalized(jl_model *m, int n, const int32_t *sess
                                          float *top_lp_out, float *logits_out) {
     return decode_impl(m, n, sessions, tokens, positions, temperatures, uniforms, next_tokens, logits_out, topkp_args(top_k, top_p),
                        logprob_args(top_n, lp_out, top_ids_out, top_lp_out), penalty_args(pen));
+}
+
+static ConstraintArgs constraint_args(int n_allow, const uint32_t *allow, const int32_t *allow_row) {
+    ConstraintArgs a;
+    a.n_allow = n_allow, a.allow = allow, a.allow_row = allow_row;
+    return a;
+}
+
+extern "C" int jl_model_sample_multi_constrained(jl_model *m, int n, const int32_t *sessions, const float *temperatures, const int32_t *top_k,
+                                                 const float *top_p, const float *uniforms, const int32_t *top_n, const jl_penalties *pen,
+                                                 int n_allow, const uint32_t *allow, const int32_t *allow_row, int32_t *tokens_out, float *lp_out,
+                                                 int32_t *top_ids_out, float *top_lp_out, float *logits_out) {
+    return sample_multi_impl(m, n, sessions, temperatures, uniforms, tokens_out, logits_out, topkp_args(top_k, top_p),
+                             logprob_args(top_n, lp_out, top_ids_out, top_lp_out), penalty_args(pen), constraint_args(n_allow, allow, allow_row));
+}
+
+extern "C" int jl_model_decode_constrained(jl_model *m, int n, const int32_t *sessions, const int32_t *tokens, const int32_t *positions,
+                                           const float *temperatures, const int32_t *top_k, const float *top_p, const float *uniforms,
+                                           const int32_t *top_n, const jl_penalties *pen, int n_allow, const uint32_t *allow,
+                                           const int32_t *allow_row, int32_t *next_tokens, float *lp_out, int32_t *top_ids_out,
+                                           float *top_lp_out, float *logits_out) {
+    return decode_impl(m, n, sessions, tokens, positions, temperatures, uniforms, next_tokens, logits_out, topkp_args(top_k, top_p),
+                       logprob_args(top_n, lp_out, top_ids_out, top_lp_out), penalty_args(pen), constraint_args(n_allow, allow, allow_row));
+}
+
+// HOST-buffer entry point for crafted rows: the selection of the model calls (penalties and masks into processed rows, the arg-max on
+// them, constrained and filtered sampled rows by the top-k / top-p kernel, the other sampled rows by the reference's rule)
+extern "C" int jl_select_constrained(jl_ctx *ctx, int n, int vocab, const float *logits, int64_t ld, const float *temperatures,
+                                     const int32_t *top_k, const float *top_p, const float *uniforms, const jl_penalties *pen, int n_allow,
+                                     const uint32_t *allow, const int32_t *allow_row, int32_t *out) {
+    if (!ctx) return JL_ERR_INVALID;
+    const char *who = "select_constrained";
+    if (n < 1 || n > 65535 || vocab < 1 || vocab > JL_TOPKP_MAX_VOCAB || ld < vocab || !logits || !out)
+        return jl_set_error(ctx, JL_ERR_INVALID, "%s: bad arguments (n=%d, vocab=%d, ld=%lld)", who, n, vocab, (long long)ld);
+    std::vector<char> filtered((size_t)n, 0);
+    int nf = 0;
+    M_CHECK(jl_topkp_check(ctx, who, n, vocab, temperatures, top_k, top_p, uniforms, filtered.data(), &nf));
+    PenaltyPlan plan;
+    M_CHECK(jl_penalty_check(ctx, who, n, vocab, pen, &plan));
+    int n_con = 0;
+    M_CHECK(jl_constraint_check(ctx, who, n, vocab, n_allow, allow, allow_row, &n_con));
+    for (int i = 0; i < n; i++) {
+        if (!temperatures || !(temperatures[i] > 0.0f)) continue;
+        if (!(uniforms[i] >= 0.0f && uniforms[i] <= 1.0f))
+            return jl_set_error(ctx, JL_ERR_INVALID, "%s: row %d: uniform %g (in [0, 1])", who, i, (double)uniforms[i]);
+        if (allow_row && allow_row[i] >= 0 && !filtered[(size_t)i]) filtered[(size_t)i] = 1, nf++;
+    }
+    const jl_penalties none = {};
+    const size_t words = (size_t)(vocab + 31) / 32;
+    std::vector<char> tab(pen ? plan.bytes : (size_t)n * sizeof(PenaltyRow));
+    jl_penalty_pack(pen ? pen : &none, n, plan, tab.data());
+    std::vector<uint32_t> mrows;
+    int nm = 0;
+    if (n_con > 0) {
+        mrows.resize((size_t)n * words);
+        nm = jl_constraint_pack(n, vocab, n_allow, allow, allow_row, tab.data(), mrows.data());
+    }
+    const bool processed = plan.n_on > 0 || n_con > 0;
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    JL_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
+    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    const size_t lb = ((size_t)(n - 1) * ld + vocab) * 4, rb = al((size_t)n * vocab * 4), tb = al(tab.size()), mb = al((size_t)nm * words * 4);
+    const size_t ob = al((size_t)n * 4), kb = al((size_t)n * sizeof(TopkpRow));
+    float *dl = (float *)jl_scratch(ctx, 0, lb);
+    char *dw = (char *)jl_scratch(ctx, 1, 3 * rb + tb + mb);
+    float *dex = (float *)jl_scratch(ctx, 2, rb);
+    char *dsel = (char *)jl_scratch(ctx, 3, ob + kb + jl_argmax_scratch_bytes(n));
+    if (!dl || !dw || !dex || !dsel) return JL_ERR_OOM;
+    unsigned *dcnt = (unsigned *)dw;
+    float *dbias = (float *)(dw + rb), *dproc = (float *)(dw + 2 * rb);
+    void *dtab = dw + 3 * rb;
+    uint32_t *dmask = (uint32_t *)(dw + 3 * rb + tb);
+    int32_t *dout = (int32_t *)dsel;
+    TopkpRow *drows = (TopkpRow *)(dsel + ob);
+    void *dargs = dsel + ob + kb;
+    cudaStream_t st = ctx->stream;
+    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(dl, logits, lb, cudaMemcpyHostToDevice, st));
+    const float *src = dl;
+    int64_t lds = ld;
+    if (processed) {
+        JL_CUDA_CHECK(ctx, cudaMemsetAsync(dcnt, 0, (size_t)n * vocab * 4, st));
+        JL_CUDA_CHECK(ctx, cudaMemcpyAsync(dtab, tab.data(), tab.size(), cudaMemcpyHostToDevice, st));
+        if (nm > 0) JL_CUDA_CHECK(ctx, cudaMemcpyAsync(dmask, mrows.data(), (size_t)nm * words * 4, cudaMemcpyHostToDevice, st));
+        M_CHECK(jl_launch_penalties(ctx, st, dl, ld, vocab, n, dtab, plan, dcnt, dbias, nm > 0 ? dmask : nullptr, dproc));
+        src = dproc, lds = vocab;
+    }
+    M_CHECK(jl_launch_argmax(ctx, st, src, n, vocab, (int)lds, dout, dargs));
+    std::vector<TopkpRow> hr;
+    for (int i = 0; i < n; i++)
+        if (filtered[(size_t)i]) hr.push_back(TopkpRow{i, temperatures[i], top_k ? top_k[i] : 0, top_p ? top_p[i] : 1.0f, uniforms[i]});
+    if (!hr.empty()) {
+        JL_CUDA_CHECK(ctx, cudaMemcpyAsync(drows, hr.data(), hr.size() * sizeof(TopkpRow), cudaMemcpyHostToDevice, st));
+        M_CHECK(jl_launch_sample_topkp(ctx, st, src, lds, vocab, drows, (int)hr.size(), dex, dout));
+    }
+    for (int i = 0; temperatures && i < n; i++) {
+        if (!(temperatures[i] > 0.0f) || filtered[(size_t)i]) continue;
+        softmax_sample_kernel<<<1, 256, 0, st>>>(src + (size_t)i * lds, dex + (size_t)i * vocab, vocab, temperatures[i], uniforms[i], dout + i);
+        ctx->launches++;
+        JL_CUDA_CHECK(ctx, cudaGetLastError());
+    }
+    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(out, dout, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+    JL_CUDA_CHECK(ctx, cudaStreamSynchronize(st));
+    return JL_OK;
 }
 
 extern "C" int jl_model_decode(jl_model *m, int n, const int32_t *sessions, const int32_t *tokens, const int32_t *positions,

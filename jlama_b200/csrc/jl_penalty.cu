@@ -9,11 +9,16 @@
 // row), bit 31 flags a prompt occurrence (atomicOr).  Integer atomics on disjoint bit fields commute, so the words are exact whatever the
 // order of the atomics.  The apply kernel (vocabulary slices x rows) reads each logit and its word, writes the processed logit, and
 // clears the words it found set, so nothing is cleared per call.  Unpenalised rows are copied.  The logits are read-only.
+//
+// Allowed-token masks (DESIGN §3.18) ride the same apply pass: a row with a mask (PenaltyRow::mask >= 0) reads one mask word per 32
+// tokens (the lanes of a warp share it) and writes -inf for every token whose bit is clear, after its penalties.  A call without a
+// masked row passes no mask and runs exactly as before.
 #include "jl_common.cuh"
 
 #include <math.h>
 
 #include <algorithm>
+#include <vector>
 
 namespace {
 
@@ -43,13 +48,14 @@ __global__ void __launch_bounds__(PEN_THREADS) penalty_mark_kernel(const Penalty
 }
 
 __global__ void __launch_bounds__(PEN_THREADS) penalty_apply_kernel(const float *logits, int64_t ld, int vocab, const PenaltyRow *rows,
-                                                                    unsigned *cnt, const float *bias, float *out) {
+                                                                    unsigned *cnt, const float *bias, const uint32_t *mask, float *out) {
     const int row = blockIdx.y;
     const PenaltyRow r = rows[row];
     const float *l = logits + (size_t)row * ld;
     float *o = out + (size_t)row * vocab;
     unsigned *c = cnt + (size_t)row * vocab;
     const float *bs = bias + (size_t)row * vocab;
+    const uint32_t *mk = mask && r.mask >= 0 ? mask + (size_t)r.mask * (size_t)((vocab + 31) / 32) : nullptr;
     const int i1 = min(vocab, (int)(blockIdx.x + 1) * PEN_SLICE);
     for (int i = blockIdx.x * PEN_SLICE + (int)threadIdx.x; i < i1; i += PEN_THREADS) {
         float v = l[i];
@@ -62,6 +68,7 @@ __global__ void __launch_bounds__(PEN_THREADS) penalty_apply_kernel(const float 
             v = __fsub_rn(v, __fmul_rn((float)k, r.frequency));
             if (k) v = __fsub_rn(v, r.presence);
         }
+        if (mk && !((mk[i >> 5] >> (i & 31)) & 1u)) v = -INFINITY;
         o[i] = v;
     }
 }
@@ -139,23 +146,69 @@ void jl_penalty_pack(const jl_penalties *pen, int n, const PenaltyPlan &plan, vo
         r.bias0 = pen->bias_off ? pen->bias_off[i] - bb : 0;
         r.bias1 = pen->bias_off ? pen->bias_off[i + 1] - bb : 0;
         r.on = r.presence != 0.0f || r.frequency != 0.0f || r.repetition != 1.0f || r.bias1 > r.bias0;
+        r.mask = -1;
     }
 }
 
 int jl_launch_penalties(jl_ctx *ctx, cudaStream_t st, const float *logits, int64_t ld, int vocab, int n, const void *tab,
-                        const PenaltyPlan &plan, unsigned *cnt, float *bias, float *out) {
+                        const PenaltyPlan &plan, unsigned *cnt, float *bias, const uint32_t *mask, float *out) {
     if (n <= 0) return JL_OK;
     if (vocab < 1 || n > 65535) return jl_set_error(ctx, JL_ERR_INVALID, "penalties: %d rows of vocabulary %d", n, vocab);
     const PenaltyRow *rows = (const PenaltyRow *)tab;
     const int32_t *hist = (const int32_t *)(rows + n), *bias_ids = hist + plan.n_hist;
     const float *bias_vals = (const float *)(bias_ids + plan.n_bias);
-    penalty_mark_kernel<<<n, PEN_THREADS, 0, st>>>(rows, hist, bias_ids, bias_vals, vocab, cnt, bias);
-    ctx->launches++;
-    JL_CUDA_CHECK(ctx, cudaGetLastError());
-    penalty_apply_kernel<<<dim3((vocab + PEN_SLICE - 1) / PEN_SLICE, n), PEN_THREADS, 0, st>>>(logits, ld, vocab, rows, cnt, bias, out);
+    if (!mask || plan.n_on > 0) { // a masked call without a penalised row has nothing to mark
+        penalty_mark_kernel<<<n, PEN_THREADS, 0, st>>>(rows, hist, bias_ids, bias_vals, vocab, cnt, bias);
+        ctx->launches++;
+        JL_CUDA_CHECK(ctx, cudaGetLastError());
+    }
+    penalty_apply_kernel<<<dim3((vocab + PEN_SLICE - 1) / PEN_SLICE, n), PEN_THREADS, 0, st>>>(logits, ld, vocab, rows, cnt, bias, mask, out);
     ctx->launches++;
     JL_CUDA_CHECK(ctx, cudaGetLastError());
     return JL_OK;
+}
+
+int jl_constraint_check(jl_ctx *ctx, const char *who, int n, int vocab, int n_allow, const uint32_t *allow, const int32_t *allow_row,
+                        int *n_on) {
+    *n_on = 0;
+    if (!allow_row) return JL_OK;
+    if (n_allow < 0) return jl_set_error(ctx, JL_ERR_INVALID, "%s: n_allow = %d is negative", who, n_allow);
+    if (n_allow > 0 && !allow) return jl_set_error(ctx, JL_ERR_INVALID, "%s: %d mask rows without allow", who, n_allow);
+    const size_t words = (size_t)(vocab + 31) / 32;
+    std::vector<char> seen((size_t)n_allow, 0); // 1: checked and not empty
+    for (int i = 0; i < n; i++) {
+        const int a = allow_row[i];
+        if (a < -1 || a >= n_allow) return jl_set_error(ctx, JL_ERR_INVALID, "%s: row %d: allow_row %d outside [-1, %d)", who, i, a, n_allow);
+        if (a < 0) continue;
+        if (!seen[(size_t)a]) {
+            const uint32_t *w = allow + (size_t)a * words;
+            bool any = false;
+            for (size_t k = 0; k < words && !any; k++) {
+                const int left = vocab - (int)(k * 32); // bits at or above vocab do not count
+                any = (left >= 32 ? w[k] : w[k] & ((1u << left) - 1u)) != 0u;
+            }
+            if (!any) return jl_set_error(ctx, JL_ERR_INVALID, "%s: row %d: mask row %d allows no token below %d", who, i, a, vocab);
+            seen[(size_t)a] = 1;
+        }
+        ++*n_on;
+    }
+    return JL_OK;
+}
+
+int jl_constraint_pack(int n, int vocab, int n_allow, const uint32_t *allow, const int32_t *allow_row, void *tab, uint32_t *dst) {
+    PenaltyRow *rows = (PenaltyRow *)tab;
+    const size_t words = (size_t)(vocab + 31) / 32;
+    std::vector<int> slot((size_t)n_allow, -1);
+    int c = 0;
+    for (int i = 0; i < n; i++) {
+        const int a = allow_row[i];
+        if (a >= 0 && slot[(size_t)a] < 0) {
+            slot[(size_t)a] = c;
+            memcpy(dst + (size_t)c++ * words, allow + (size_t)a * words, words * 4);
+        }
+        rows[i].mask = a >= 0 ? slot[(size_t)a] : -1;
+    }
+    return c;
 }
 
 // HOST-buffer entry point for crafted rows
@@ -184,7 +237,7 @@ extern "C" int jl_apply_penalties(jl_ctx *ctx, int n, int vocab, const float *lo
     JL_CUDA_CHECK(ctx, cudaMemcpyAsync(dl, logits, lb, cudaMemcpyHostToDevice, ctx->stream));
     JL_CUDA_CHECK(ctx, cudaMemsetAsync(dcnt, 0, rb, ctx->stream));
     JL_CUDA_CHECK(ctx, cudaMemcpyAsync(dtab, tab.data(), tab.size(), cudaMemcpyHostToDevice, ctx->stream));
-    const int rc = jl_launch_penalties(ctx, ctx->stream, dl, ld, vocab, n, dtab, p, dcnt, dbias, dout);
+    const int rc = jl_launch_penalties(ctx, ctx->stream, dl, ld, vocab, n, dtab, p, dcnt, dbias, nullptr, dout);
     if (rc != JL_OK) return rc;
     JL_CUDA_CHECK(ctx, cudaMemcpyAsync(out, dout, rb, cudaMemcpyDeviceToHost, ctx->stream));
     JL_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));

@@ -37,7 +37,8 @@
 
 #include "../../include/jlama_b200.h"
 
-void jl_model_limits(jl_model *m, int out[5]); // jl_model.cu: {max_sessions, max_context, max_batch, max rows per decode call, ctx_per_page}
+void jl_model_limits(jl_model *m, int out[6]); // jl_model.cu: {max_sessions, max_context, max_batch, max rows per decode call, ctx_per_page,
+                                               // vocab_size}
 
 namespace {
 
@@ -116,6 +117,9 @@ struct jl_sched {
     jl_sched_topkp_backend tb = {}; // optional: calls with a top-k / top-p filtered row
     jl_sched_logprob_backend lb = {}; // optional: calls with a logprob request
     jl_sched_penalty_backend pb = {}; // optional: calls with a penalised request
+    jl_sched_constraint_backend cb = {}; // optional: calls with a constrained request, with the mask provider below
+    jl_sched_mask_fn *mask_fn = nullptr;
+    void *mask_user = nullptr;
     jl_sched_fork_backend fb = {};    // optional: n completions of one prompt
     jl_model *model = nullptr;        // jl_sched_create: the model behind the backend
     // prefix cache (DESIGN §3.17), on when prefix_max_pages > 0; entries and index change under `mu`, their handles outside it
@@ -233,6 +237,27 @@ static int mb_sample_multi_topkp(void *u, int n, const int32_t *sessions, const 
     return jl_model_sample_multi_topkp((jl_model *)u, n, sessions, temperatures, top_k, top_p, uniforms, tokens, nullptr);
 }
 
+extern "C" int jl_model_decode_constrained(jl_model *, int, const int32_t *, const int32_t *, const int32_t *, const float *, const int32_t *,
+                                           const float *, const float *, const int32_t *, const jl_penalties *, int, const uint32_t *,
+                                           const int32_t *, int32_t *, float *, int32_t *, float *, float *) __attribute__((weak));
+extern "C" int jl_model_sample_multi_constrained(jl_model *, int, const int32_t *, const float *, const int32_t *, const float *, const float *,
+                                                 const int32_t *, const jl_penalties *, int, const uint32_t *, const int32_t *, int32_t *, float *,
+                                                 int32_t *, float *, float *) __attribute__((weak));
+static int mb_decode_constrained(void *u, int n, const int32_t *sessions, const int32_t *tokens, const int32_t *positions,
+                                 const float *temperatures, const int32_t *top_k, const float *top_p, const float *uniforms, const int32_t *top_n,
+                                 const jl_penalties *pen, int n_allow, const uint32_t *allow, const int32_t *allow_row, int32_t *next, float *lp,
+                                 int32_t *top_ids, float *top_lp) {
+    return jl_model_decode_constrained((jl_model *)u, n, sessions, tokens, positions, temperatures, top_k, top_p, uniforms, top_n, pen, n_allow,
+                                       allow, allow_row, next, lp, top_ids, top_lp, nullptr);
+}
+static int mb_sample_multi_constrained(void *u, int n, const int32_t *sessions, const float *temperatures, const int32_t *top_k,
+                                       const float *top_p, const float *uniforms, const int32_t *top_n, const jl_penalties *pen, int n_allow,
+                                       const uint32_t *allow, const int32_t *allow_row, int32_t *tokens, float *lp, int32_t *top_ids,
+                                       float *top_lp) {
+    return jl_model_sample_multi_constrained((jl_model *)u, n, sessions, temperatures, top_k, top_p, uniforms, top_n, pen, n_allow, allow,
+                                             allow_row, tokens, lp, top_ids, top_lp, nullptr);
+}
+
 extern "C" int jl_model_kv_fork(jl_model *, int, int, int, const int32_t *) __attribute__((weak));
 static int mb_fork(void *u, int src, int positions, int n, const int32_t *dst) { return jl_model_kv_fork((jl_model *)u, src, positions, n, dst); }
 
@@ -280,7 +305,7 @@ extern "C" int jl_sched_create_backend(const jl_sched_backend *be, void *user, i
 
 extern "C" int jl_sched_create(jl_model *m, int max_active, int prefill_tokens_per_step, jl_sched **out) {
     if (!m || !out) return JL_ERR_INVALID;
-    int lim[5] = {0, 0, 0, 0, 0};
+    int lim[6] = {0, 0, 0, 0, 0, 0};
     jl_model_limits(m, lim);
     if (lim[0] <= 0) return JL_ERR_INVALID; // not finalized
     const int n = max_active > 0 && max_active < lim[0] ? max_active : lim[0];
@@ -291,6 +316,8 @@ extern "C" int jl_sched_create(jl_model *m, int max_active, int prefill_tokens_p
     if (rc == JL_OK && jl_model_decode_logprobs && jl_model_sample_multi_logprobs) (*out)->lb = {mb_decode_logprobs, mb_sample_multi_logprobs};
     if (rc == JL_OK && jl_model_decode_penalized && jl_model_sample_multi_penalized)
         (*out)->pb = {mb_decode_penalized, mb_sample_multi_penalized};
+    if (rc == JL_OK && jl_model_decode_constrained && jl_model_sample_multi_constrained)
+        (*out)->cb = {mb_decode_constrained, mb_sample_multi_constrained, lim[5]};
     if (rc == JL_OK && jl_model_kv_fork) (*out)->fb = {mb_fork};
     if (rc == JL_OK) (*out)->model = m;
     return rc;
@@ -332,6 +359,24 @@ extern "C" int jl_sched_set_penalty_backend(jl_sched *s, const jl_sched_penalty_
     return JL_OK;
 }
 
+extern "C" int jl_sched_set_constraint_backend(jl_sched *s, const jl_sched_constraint_backend *cb) {
+    if (!s || !cb || !cb->decode_constrained || !cb->sample_multi_constrained || cb->vocab < 1) return JL_ERR_INVALID;
+    std::lock_guard<std::mutex> a(s->step_mu);
+    std::lock_guard<std::mutex> lk(s->mu);
+    if (s->step_no > 0) return sched_error(s, JL_ERR_INVALID, "set_constraint_backend: the scheduler has already stepped");
+    s->cb = *cb;
+    return JL_OK;
+}
+
+extern "C" int jl_sched_set_mask_provider(jl_sched *s, jl_sched_mask_fn *fn, void *user) {
+    if (!s) return JL_ERR_INVALID;
+    std::lock_guard<std::mutex> a(s->step_mu);
+    std::lock_guard<std::mutex> lk(s->mu);
+    if (s->step_no > 0) return sched_error(s, JL_ERR_INVALID, "set_mask_provider: the scheduler has already stepped");
+    s->mask_fn = fn, s->mask_user = fn ? user : nullptr;
+    return JL_OK;
+}
+
 extern "C" int jl_sched_set_fork_backend(jl_sched *s, const jl_sched_fork_backend *fb) {
     if (!s || !fb || !fb->fork) return JL_ERR_INVALID;
     std::lock_guard<std::mutex> a(s->step_mu);
@@ -348,7 +393,7 @@ extern "C" int jl_sched_set_prefix_cache(jl_sched *s, const jl_sched_prefix_back
         if (!pb->retain || !pb->attach || !pb->release || !pb->retained || pb->ctx_per_page < 1) return JL_ERR_INVALID;
         xb = *pb;
     } else if (s->model && jl_model_kv_retain) {
-        int lim[5] = {0, 0, 0, 0, 0};
+        int lim[6] = {0, 0, 0, 0, 0, 0};
         jl_model_limits(s->model, lim);
         xb = {mb_retain, mb_attach, mb_release, mb_retained, lim[4]};
     }
@@ -541,6 +586,9 @@ static int make_request(jl_sched *s, Request &r, const int32_t *prompt, int n_pr
         return sched_error(s, -1, "submit: top_k / top_p need the top-k / top-p backend (jl_sched_set_topkp_backend)");
     if (logprobs >= 0 && !s->lb.decode_logprobs)
         return sched_error(s, -1, "submit: logprobs need the logprob backend (jl_sched_set_logprob_backend)");
+    if ((flags & JL_SCHED_CONSTRAINED) && (!s->mask_fn || !s->cb.decode_constrained))
+        return sched_error(s, -1, "submit: constrained requests need a mask provider and the constraint backend (jl_sched_set_mask_provider, "
+                                  "jl_sched_set_constraint_backend)");
     if (continue_request >= 0) {
         // AbstractModel.generate :533 startPos = kvmem.getCurrentContextPosition(): a follow-up on the same session appends to its KV
         auto it = s->reqs.find(continue_request);
@@ -807,6 +855,8 @@ struct Select {
     const Penalty *pen = nullptr; // penalised request: its penalties, history = hist, whose first n_prompt tokens are its prompt
     std::vector<int32_t> hist;
     int n_prompt = 0;
+    bool constrained = false;     // JL_SCHED_CONSTRAINED request: `allow` is its provider's mask for this selection
+    std::vector<uint32_t> allow;
 };
 struct PrefillJob {
     int64_t id;
@@ -822,6 +872,7 @@ struct PrefillJob {
     SlotJob slot;
     std::vector<int32_t> tokens;
     int rc = JL_OK;            // status of the job's backend calls
+    std::string mask_error;    // the mask provider refused its first token
     size_t call = 0, row = 0;  // its first token: row `row` of its group's first-token call `call`
 };
 
@@ -844,16 +895,21 @@ struct PenCall {
     }
 };
 
-// the backend pair that serves a sampling call: the penalty pair when one of its rows is penalised, else the logprob pair when one wants
-// logprobs, else the top-k / top-p pair when one is filtered, else the plain calls
-enum Tier { PLAIN, TOPKP, LOGPROB, PENALTY };
-Tier tier_of(const Select &x) { return x.pen ? PENALTY : x.logprobs >= 0 ? LOGPROB : x.filtered ? TOPKP : PLAIN; }
+// the backend pair that serves a sampling call: the constraint pair when one of its rows is constrained, else the penalty pair when one
+// is penalised, else the logprob pair when one wants logprobs, else the top-k / top-p pair when one is filtered, else the plain calls
+enum Tier { PLAIN, TOPKP, LOGPROB, PENALTY, CONSTRAINED };
+Tier tier_of(const Select &x) {
+    return x.constrained ? CONSTRAINED : x.pen ? PENALTY : x.logprobs >= 0 ? LOGPROB : x.filtered ? TOPKP : PLAIN;
+}
 
 // the arguments and outputs of one sampling call (first tokens, or a decode step with its tokens and positions), row by row
 struct Call {
     std::vector<int32_t> sessions, tokens, positions, top_k, top_n;
     std::vector<float> temperatures, uniforms, top_p;
     PenCall pc;
+    std::vector<uint32_t> allow;    // the mask rows of the constrained rows, one each
+    std::vector<int32_t> allow_row; // row -> its mask row, -1 = unconstrained
+    int n_allow = 0;
     Tier tier = PLAIN;
     std::vector<int32_t> next, top_ids; // the tokens; logprob and penalty calls also fill lp, top_ids and top_lp
     std::vector<float> lp, top_lp;
@@ -862,6 +918,8 @@ struct Call {
         sessions.push_back(session), temperatures.push_back(x.temperature), uniforms.push_back(x.uniform);
         top_k.push_back(x.top_k), top_p.push_back(x.top_p), top_n.push_back(x.logprobs);
         pc.add(x.pen, x.hist, x.n_prompt);
+        allow_row.push_back(x.constrained ? n_allow++ : -1);
+        if (x.constrained) allow.insert(allow.end(), x.allow.begin(), x.allow.end());
         tier = std::max(tier, tier_of(x));
     }
     // row i's logprobs -> the request's streams
@@ -1093,6 +1151,7 @@ static void plan(jl_sched *s, Step &p) {
             if (r.filtered()) j.sel.top_k = r.top_k, j.sel.top_p = r.top_p, j.sel.filtered = true;
             j.sel.logprobs = r.logprobs;
             if (r.pen.on()) j.sel.pen = &r.pen, j.sel.hist = r.prompt, j.sel.n_prompt = (int)r.prompt.size();
+            j.sel.constrained = (r.flags & JL_SCHED_CONSTRAINED) != 0;
         }
         jobs.push_back(std::move(j));
     }
@@ -1114,10 +1173,39 @@ static void fork_group(jl_sched *s, Step &p, size_t k) {
     if (p.first_error == JL_OK) p.first_error = sched_error(s, rc, "request %lld: fork into %zu siblings failed (%d)", (long long)j.id, dst.size(), rc);
 }
 
+// the provider's mask for one selection of a constrained request (table unlocked: the provider may call back into the scheduler);
+// false with the reason when it fails or allows no token below the vocabulary
+static bool mask_for(jl_sched *s, int64_t id, const std::vector<int32_t> &generated, std::vector<uint32_t> &allow, std::string &why) {
+    const int V = s->cb.vocab;
+    allow.assign((size_t)(V + 31) / 32, 0u);
+    const int rc = s->mask_fn(s->mask_user, id, generated.data(), (int)generated.size(), allow.data());
+    if (rc != 0) {
+        why = "the mask provider failed (" + std::to_string(rc) + ")";
+        return false;
+    }
+    for (size_t k = 0; k < allow.size(); k++) {
+        const int left = V - (int)(k * 32);
+        if ((left >= 32 ? allow[k] : allow[k] & ((1u << left) - 1u)) != 0u) return true;
+    }
+    why = "the mask provider allowed no token";
+    return false;
+}
+
+// must hold s->mu.  A constrained request whose provider refused its selection fails alone.
+static void mask_failed(jl_sched *s, Step &p, Request &r, const std::string &why) {
+    const int rc = sched_error(s, JL_ERR_INVALID, "request %lld: %s", (long long)r.id, why.c_str());
+    if (p.first_error == JL_OK) p.first_error = rc;
+    finish(s, r, JL_SCHED_FAILED, JL_FINISH_ERROR), p.st.finished++;
+}
+
 // the first tokens of completed prompts (table unlocked); without a batch backend a plain call has one row
 static int sample_first(jl_sched *s, Call &c) {
     const int n = (int)c.sessions.size();
     const jl_penalties pen = c.pc.get();
+    if (c.tier == CONSTRAINED)
+        return s->cb.sample_multi_constrained(s->user, n, c.sessions.data(), c.temperatures.data(), c.top_k.data(), c.top_p.data(),
+                                              c.uniforms.data(), c.top_n.data(), &pen, c.n_allow, c.allow.data(), c.allow_row.data(),
+                                              c.next.data(), c.lp.data(), c.top_ids.data(), c.top_lp.data());
     if (c.tier == PENALTY)
         return s->pb.sample_multi_penalized(s->user, n, c.sessions.data(), c.temperatures.data(), c.top_k.data(), c.top_p.data(), c.uniforms.data(),
                                             c.top_n.data(), &pen, c.next.data(), c.lp.data(), c.top_ids.data(), c.top_lp.data());
@@ -1158,6 +1246,7 @@ static void apply(jl_sched *s, Step &p, const PrefillJob &j, const std::vector<C
         finish(s, r, JL_SCHED_FINISHED, JL_FINISH_CANCELLED), st.finished++;
         return;
     }
+    if (!j.mask_error.empty()) return mask_failed(s, p, r, j.mask_error);
     const Call &c = calls[j.call];
     r.out.push_back(c.next[j.row]);
     if (r.logprobs >= 0) c.append_lp(r, j.row);
@@ -1204,6 +1293,14 @@ static void run_group(jl_sched *s, Step &p, size_t b, size_t e) {
         if (j.rc == JL_OK && !j.dropped && !j.retain.empty()) prefix_retain(s, j.session, j.retain);
         if (j.rc == JL_OK && j.last && !j.cancelled && !j.dropped) done.push_back(k);
     }
+    // the masks of the constrained first tokens (n_generated 0); a refused one leaves the call
+    const std::vector<int32_t> none;
+    done.erase(std::remove_if(done.begin(), done.end(),
+                              [&](size_t k) {
+                                  PrefillJob &j = jobs[k];
+                                  return j.sel.constrained && !mask_for(s, j.id, none, j.sel.allow, j.mask_error);
+                              }),
+               done.end());
     std::vector<Call> calls;
     for (size_t g = 0; g < done.size(); g += (size_t)s->max_rows) {
         const size_t n = std::min(done.size() - g, (size_t)s->max_rows);
@@ -1240,6 +1337,10 @@ static void run_prompts(jl_sched *s, Step &p) {
 static int decode_call(jl_sched *s, Call &c) {
     const int n = (int)c.sessions.size();
     const jl_penalties pen = c.pc.get();
+    if (c.tier == CONSTRAINED)
+        return s->cb.decode_constrained(s->user, n, c.sessions.data(), c.tokens.data(), c.positions.data(), c.temperatures.data(), c.top_k.data(),
+                                        c.top_p.data(), c.uniforms.data(), c.top_n.data(), &pen, c.n_allow, c.allow.data(), c.allow_row.data(),
+                                        c.next.data(), c.lp.data(), c.top_ids.data(), c.top_lp.data());
     if (c.tier == PENALTY)
         return s->pb.decode_penalized(s->user, n, c.sessions.data(), c.tokens.data(), c.positions.data(), c.temperatures.data(), c.top_k.data(),
                                       c.top_p.data(), c.uniforms.data(), c.top_n.data(), &pen, c.next.data(), c.lp.data(), c.top_ids.data(),
@@ -1258,8 +1359,14 @@ static int decode_call(jl_sched *s, Call &c) {
 static void run_decode(jl_sched *s, Step &p) {
     jl_sched_stats &st = p.st;
     const size_t M = (size_t)s->max_rows;
-    std::vector<Call> calls;
-    std::vector<int64_t> ids; // request of row i of call g: ids[g * max_rows + i]
+    struct Row {
+        int64_t id;
+        int32_t session, token, position;
+        Select x;
+        std::vector<int32_t> generated; // constrained: a copy for the mask provider
+        std::string refused;
+    };
+    std::vector<Row> rows;
     {
         std::lock_guard<std::mutex> lk(s->mu);
         for (int64_t id : s->active) {
@@ -1271,11 +1378,28 @@ static void run_decode(jl_sched *s, Step &p) {
                 x.hist = r.prompt;
                 x.hist.insert(x.hist.end(), r.out.begin(), r.out.end());
             }
-            if (ids.size() % M == 0) calls.emplace_back(M);
-            Call &c = calls.back();
-            c.add(r.session, x), c.tokens.push_back(r.out.back()), c.positions.push_back(r.next_pos());
-            ids.push_back(id);
+            x.constrained = (r.flags & JL_SCHED_CONSTRAINED) != 0;
+            rows.push_back(Row{id, r.session, r.out.back(), r.next_pos(), std::move(x), {}, {}});
+            if (rows.back().x.constrained) rows.back().generated = r.out;
         }
+    }
+    // the masks of the constrained rows; a refused row fails its request and leaves the step
+    bool refused = false;
+    for (Row &w : rows)
+        if (w.x.constrained && !mask_for(s, w.id, w.generated, w.x.allow, w.refused)) refused = true;
+    if (refused) {
+        std::lock_guard<std::mutex> lk(s->mu);
+        for (const Row &w : rows)
+            if (!w.refused.empty()) mask_failed(s, p, s->reqs[w.id], w.refused);
+    }
+    std::vector<Call> calls;
+    std::vector<int64_t> ids; // request of row i of call g: ids[g * max_rows + i]
+    for (const Row &w : rows) {
+        if (!w.refused.empty()) continue;
+        if (ids.size() % M == 0) calls.emplace_back(M);
+        Call &c = calls.back();
+        c.add(w.session, w.x), c.tokens.push_back(w.token), c.positions.push_back(w.position);
+        ids.push_back(w.id);
     }
     for (size_t g = 0; g < calls.size(); g++) {
         Call &c = calls[g];

@@ -82,6 +82,25 @@ def _bias_pairs(logit_bias):
     return np.asarray([t for t, _ in pairs], dtype=np.int32), np.asarray([v for _, v in pairs], dtype=np.float32)
 
 
+def _mask_arrays(allowed, n, vocab):
+    """per-row allowed sets (None = unconstrained; a bool[vocab] or packed uint32 words, DESIGN §3.18) -> (n_allow, allow
+    [n_allow][words] uint32, allow_row int32[n])"""
+    from .sampling import mask_words, pack_mask
+    assert len(allowed) == n
+    words = mask_words(vocab)
+    rows, allow_row = [], np.full(n, -1, dtype=np.int32)
+    for i, a in enumerate(allowed):
+        if a is None:
+            continue
+        a = np.asarray(a)
+        w = pack_mask(a) if a.dtype == bool else np.asarray(a, dtype=np.uint32).reshape(-1)
+        assert len(w) == words, (i, len(w), words)
+        allow_row[i] = len(rows)
+        rows.append(w)
+    allow = np.ascontiguousarray(np.concatenate(rows) if rows else np.zeros(words, np.uint32), dtype=np.uint32)
+    return len(rows), allow, allow_row
+
+
 def _penalty_struct(penalties, n):
     """per-row RowPenalty (None = unpenalised) -> (native.Penalties, the arrays it points into, to keep alive for the call)"""
     rows = [RowPenalty() if q is None else RowPenalty(*q) for q in penalties]
@@ -252,12 +271,13 @@ class LlamaModel:
         self.ctx.check(self.lib.jl_model_batch_forward_multi(self.h, len(segments), ptr(sessions), ptr(starts), ptr(lengths), ptr(tokens)))
 
     def sample_multi(self, sessions, temperatures=None, uniforms=None, want_logits=False, top_k=None, top_p=None, logprobs=None,
-                     penalties=None):
+                     penalties=None, allowed=None):
         """AbstractModel.sample on the last forwarded row of each session, in one lm_head pass; rows with a temperature other than 0
         draw with the reference's rule from uniforms[i], or with the top-k / top-p rule (DESIGN §3.12) when top_k / top_p (per row)
         filter them.  Returns (tokens, raw logits [n, vocab] or None); with logprobs (an int or one per row: -1 none, 0 the chosen
         token's, up to 20 alternatives; DESIGN §3.13) also a TokenLogprobs of the chosen tokens.  penalties: one RowPenalty (or None)
-        per row (DESIGN §3.14); each row is then selected from its processed logits."""
+        per row (DESIGN §3.14); each row is then selected from its processed logits.  allowed: per row None or the allowed-token set
+        (a bool[vocab] or packed uint32 words, DESIGN §3.18) the row is selected under; logits and logprobs stay those of the raw logits."""
         sessions = np.ascontiguousarray(sessions, dtype=np.int32)
         n = len(sessions)
         t = None if temperatures is None else np.ascontiguousarray(temperatures, dtype=np.float32)
@@ -265,6 +285,16 @@ class LlamaModel:
         assert (t is None or len(t) == n) and (u is None or len(u) == n)
         out = np.empty(n, dtype=np.int32)
         logits = np.empty((n, self.cfg["vocab"]), dtype=np.float32) if want_logits else None
+        if allowed is not None:
+            k, p = _filter_arrays(top_k, top_p, n)
+            tn = np.ascontiguousarray(np.broadcast_to(-1 if logprobs is None else logprobs, (n,)), dtype=np.int32)
+            lp = _logprob_arrays(n)
+            pen, _keep = _penalty_struct(penalties if penalties is not None else [None] * n, n)
+            n_allow, allow, allow_row = _mask_arrays(allowed, n, self.cfg["vocab"])
+            self.ctx.check(self.lib.jl_model_sample_multi_constrained(self.h, n, ptr(sessions), ptr(t), ptr(k), ptr(p), ptr(u), ptr(tn),
+                                                                      C.addressof(pen), n_allow, ptr(allow), ptr(allow_row), ptr(out),
+                                                                      ptr(lp.lp), ptr(lp.top_ids), ptr(lp.top_lp), ptr(logits)))
+            return (out, logits) if logprobs is None else (out, logits, lp)
         if penalties is not None:
             k, p = _filter_arrays(top_k, top_p, n)
             tn = np.ascontiguousarray(np.broadcast_to(-1 if logprobs is None else logprobs, (n,)), dtype=np.int32)
@@ -289,18 +319,32 @@ class LlamaModel:
         return out, logits
 
     def decode(self, tokens, positions, sessions=None, want_logits=False, temperatures=None, uniforms=None, top_k=None, top_p=None,
-               logprobs=None, penalties=None):
+               logprobs=None, penalties=None, allowed=None):
         """One decode step for n sessions.  temperatures / uniforms (per row): rows with a temperature other than 0 are sampled with
         AbstractModel.sample's rule (:475-489) from their logits row, the others take the arg-max.  top_k / top_p (per row, optional):
         rows with a temperature above 0 that they filter are drawn with the top-k / top-p rule (DESIGN §3.12) instead.  Returns
         (next tokens, logits or None); with logprobs (an int or one per row, as in sample_multi) also a TokenLogprobs of the chosen
-        tokens.  penalties: one RowPenalty (or None) per row (DESIGN §3.14); logits and logprobs stay those of the raw logits."""
+        tokens.  penalties: one RowPenalty (or None) per row (DESIGN §3.14); logits and logprobs stay those of the raw logits.  allowed:
+        per row None or the allowed-token set the row is selected under (as in sample_multi; DESIGN §3.18)."""
         tokens = np.ascontiguousarray(tokens, dtype=np.int32)
         positions = np.ascontiguousarray(positions, dtype=np.int32)
         n = len(tokens)
         sessions = np.arange(n, dtype=np.int32) if sessions is None else np.ascontiguousarray(sessions, dtype=np.int32)
         nxt = np.empty(n, dtype=np.int32)
         logits = np.empty((n, self.cfg["vocab"]), dtype=np.float32) if want_logits else None
+        if allowed is not None:
+            t = None if temperatures is None else np.ascontiguousarray(temperatures, dtype=np.float32)
+            u = None if uniforms is None else np.ascontiguousarray(uniforms, dtype=np.float32)
+            assert (t is None or len(t) == n) and (u is None or len(u) == n)
+            k, p = _filter_arrays(top_k, top_p, n)
+            tn = np.ascontiguousarray(np.broadcast_to(-1 if logprobs is None else logprobs, (n,)), dtype=np.int32)
+            lp = _logprob_arrays(n)
+            pen, _keep = _penalty_struct(penalties if penalties is not None else [None] * n, n)
+            n_allow, allow, allow_row = _mask_arrays(allowed, n, self.cfg["vocab"])
+            self.ctx.check(self.lib.jl_model_decode_constrained(self.h, n, ptr(sessions), ptr(tokens), ptr(positions), ptr(t), ptr(k), ptr(p),
+                                                                ptr(u), ptr(tn), C.addressof(pen), n_allow, ptr(allow), ptr(allow_row), ptr(nxt),
+                                                                ptr(lp.lp), ptr(lp.top_ids), ptr(lp.top_lp), ptr(logits)))
+            return (nxt, logits) if logprobs is None else (nxt, logits, lp)
         if penalties is not None:
             t = None if temperatures is None else np.ascontiguousarray(temperatures, dtype=np.float32)
             u = None if uniforms is None else np.ascontiguousarray(uniforms, dtype=np.float32)

@@ -134,6 +134,27 @@ class SchedPenaltyBackend(C.Structure):
     _fields_ = [("decode_penalized", SCHED_DECODE_PENALIZED_FN), ("sample_multi_penalized", SCHED_SAMPLE_MULTI_PENALIZED_FN)]
 
 
+# jl_sched_constraint_backend: the calls with a constrained request (jl_model_decode_constrained / jl_model_sample_multi_constrained) and
+# the vocabulary of their masks
+SCHED_DECODE_CONSTRAINED_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                          C.POINTER(C.c_float), C.POINTER(C.c_int32), C.POINTER(C.c_float), C.POINTER(C.c_float),
+                                          C.POINTER(C.c_int32), C.POINTER(Penalties), C.c_int, C.POINTER(C.c_uint32), C.POINTER(C.c_int32),
+                                          C.POINTER(C.c_int32), C.POINTER(C.c_float), C.POINTER(C.c_int32), C.POINTER(C.c_float))
+SCHED_SAMPLE_MULTI_CONSTRAINED_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_float), C.POINTER(C.c_int32),
+                                                C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_int32), C.POINTER(Penalties), C.c_int,
+                                                C.POINTER(C.c_uint32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_float),
+                                                C.POINTER(C.c_int32), C.POINTER(C.c_float))
+
+
+class SchedConstraintBackend(C.Structure):
+    _fields_ = [("decode_constrained", SCHED_DECODE_CONSTRAINED_FN), ("sample_multi_constrained", SCHED_SAMPLE_MULTI_CONSTRAINED_FN),
+                ("vocab", C.c_int)]
+
+
+# jl_sched_mask_fn: the mask provider of constrained requests (user, request, generated, n_generated, allow_out)
+SCHED_MASK_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int64, C.POINTER(C.c_int32), C.c_int, C.POINTER(C.c_uint32))
+
+
 # jl_sched_fork_backend: n completions of one prompt (jl_model_kv_fork)
 SCHED_FORK_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int32))
 
@@ -161,6 +182,7 @@ class SchedPrefixStats(C.Structure):
 SCHED_QUEUED, SCHED_PREFILL, SCHED_DECODING, SCHED_FINISHED, SCHED_FAILED = range(5)
 FINISH_NONE, FINISH_MAX_TOKENS, FINISH_STOP_TOKEN, FINISH_CANCELLED, FINISH_ERROR = range(5)
 SCHED_KEEP_SESSION = 1
+SCHED_CONSTRAINED = 2
 
 # every symbol include/jlama_b200.h declares: (restype, argtypes)
 _vp, _i, _i64, _f, _d = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_double
@@ -243,6 +265,9 @@ SIGNATURES = {
     "jl_model_sample_multi_penalized": (_i, [_vp, _i] + [_vp] * 12),
     "jl_model_generate_penalized": (_i, [_vp, _i, _vp, _i, _i, _f, _i, _f, _vp, _i, _f, _f, _f, _i] + [_vp] * 7),
     "jl_apply_penalties": (_i, [_vp, _i, _i, _vp, _i64, _vp, _vp]),
+    "jl_model_decode_constrained": (_i, [_vp, _i] + [_vp] * 9 + [_i] + [_vp] * 7),
+    "jl_model_sample_multi_constrained": (_i, [_vp, _i] + [_vp] * 7 + [_i] + [_vp] * 7),
+    "jl_select_constrained": (_i, [_vp, _i, _i, _vp, _i64] + [_vp] * 5 + [_i] + [_vp] * 3),
     "jl_moe_route": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),
     "jl_model_decode_resident": (_i, [_vp, _i, C.c_int32, _i, _i, _vp]),
     "jl_model_read_kv": (_i, [_vp, _i, _i, _i, _i, _vp]),
@@ -271,6 +296,8 @@ SIGNATURES = {
     "jl_sched_set_logprob_backend": (_i, [_vp, C.POINTER(SchedLogprobBackend)]),
     "jl_sched_set_penalty_backend": (_i, [_vp, C.POINTER(SchedPenaltyBackend)]),
     "jl_sched_set_fork_backend": (_i, [_vp, C.POINTER(SchedForkBackend)]),
+    "jl_sched_set_constraint_backend": (_i, [_vp, C.POINTER(SchedConstraintBackend)]),
+    "jl_sched_set_mask_provider": (_i, [_vp, _vp, _vp]),  # the provider: a SCHED_MASK_FN
     "jl_sched_set_prefix_cache": (_i, [_vp, C.POINTER(SchedPrefixBackend), _i]),
     "jl_sched_prefix_stats": (_i, [_vp, C.POINTER(SchedPrefixStats)]),
     "jl_sched_request_cached": (_i, [_vp, _i64]),

@@ -94,3 +94,38 @@ def apply_penalties(row, prompt_ids=(), generated_ids=(), presence=0.0, frequenc
         b = b - c.astype(np.float32) * f
         b = np.where(c > 0, b - p, b).astype(np.float32)
     return b
+
+
+def mask_words(vocab):
+    """the uint32 words of one allowed-token mask row: (vocab + 31) // 32"""
+    return (int(vocab) + 31) // 32
+
+
+def pack_mask(allowed):
+    """bool[V] -> uint32[(V + 31) // 32]: token t is allowed when bit t % 32 of word t // 32 is set (DESIGN §3.18)"""
+    a = np.asarray(allowed, dtype=bool).reshape(-1)
+    bits = np.zeros(mask_words(len(a)) * 32, dtype=np.uint64)
+    bits[:len(a)] = a
+    return (bits.reshape(-1, 32) << np.arange(32, dtype=np.uint64)).sum(axis=1).astype(np.uint32)
+
+
+def unpack_mask(words, vocab):
+    """uint32 words -> bool[vocab]; bits at or above vocab are ignored"""
+    w = np.asarray(words, dtype=np.uint32).reshape(-1)
+    return ((w[:, None] >> np.arange(32, dtype=np.uint32)) & 1).astype(bool).reshape(-1)[:int(vocab)]
+
+
+def apply_mask(row, allowed):
+    """The constrained processed row (DESIGN §3.18): p_t = row_t where t is allowed, else -inf.  `row` is the raw row or the processed row
+    of apply_penalties; `allowed` a bool[V] or the packed uint32 words of pack_mask."""
+    l = np.asarray(row, dtype=np.float32)
+    a = np.asarray(allowed)
+    if a.dtype != bool:
+        a = unpack_mask(a, len(l))
+    return np.where(a, l, np.float32(-np.inf)).astype(np.float32)
+
+
+def select_constrained(row, allowed, temperature, top_k=0, top_p=1.0, uniform=0.0):
+    """The token of one constrained row: temperature 0 takes the arg-max of the masked row (first index on ties); otherwise the top-k /
+    top-p rule of sample_topkp draws from it, which gives a banned token weight 0 and never draws one."""
+    return sample_topkp(apply_mask(row, allowed), temperature, top_k, top_p, uniform)

@@ -48,31 +48,72 @@ def penalty_rows(pen, n):
     return out
 
 
+def allowed_rows(n_allow, allow, allow_row, n, vocab):
+    """the masks of a constrained call (ctypes pointers) -> per row None (unconstrained) or its allowed set as bool[vocab]"""
+    from .sampling import mask_words, unpack_mask
+    rows = np.ctypeslib.as_array(allow_row, shape=(n,)).copy()
+    words = np.ctypeslib.as_array(allow, shape=(n_allow * mask_words(vocab),)).copy() if n_allow else np.empty(0, np.uint32)
+    W = mask_words(vocab)
+    return [None if r < 0 else unpack_mask(words[r * W:(r + 1) * W], vocab) for r in rows]
+
+
+def _flags(keep_session, constrained):
+    return (native.SCHED_KEEP_SESSION if keep_session else 0) | (native.SCHED_CONSTRAINED if constrained else 0)
+
+
 class SessionScheduler:
-    def __init__(self, model, max_active=0, prefill_tokens_per_step=0, prefix_cache_pages=0):
+    def __init__(self, model, max_active=0, prefill_tokens_per_step=0, prefix_cache_pages=0, mask_provider=None):
         """prefix_cache_pages > 0: fresh requests reuse the KV pages of earlier prompts that share a whole-page prefix with theirs,
-        the cache holding at most that many pages no session holds (DESIGN §3.17)."""
+        the cache holding at most that many pages no session holds (DESIGN §3.17).  mask_provider: the grammar engine of constrained
+        requests (submit(..., constrained=True); DESIGN §3.18), see _install_mask_provider."""
         self.lib = model.lib
         self._model = model  # the scheduler borrows the model: keep it alive
         self._keep = None
+        self.backend_errors = []
         h = C.c_void_p()
         rc = self.lib.jl_sched_create(model.h, max_active, prefill_tokens_per_step, C.byref(h))
         if rc != native.JL_OK:
             raise native.JlamaNativeError(rc, "jl_sched_create failed (is the model finalized?)")
         self.h = h
-        if prefix_cache_pages:
-            try:
+        try:
+            if prefix_cache_pages:
                 self._check(self.lib.jl_sched_set_prefix_cache(self.h, None, int(prefix_cache_pages)))
-            except native.JlamaNativeError:
-                self.close()
-                raise
+            if mask_provider is not None:
+                self._install_mask_provider(mask_provider, int(model.cfg["vocab"]))
+        except native.JlamaNativeError:
+            self.close()
+            raise
+
+    def _install_mask_provider(self, mask_provider, vocab):
+        """mask_provider(request, generated: np.int32[k]) -> the allowed set of the request's next token, a bool[vocab] or packed uint32
+        words (sampling.pack_mask).  Called once before every selection of a constrained request, with the tokens it has generated so
+        far (none for its first token), on the stepping thread; it may call result() / cancel() but must not step.  A raised exception
+        fails that request alone (JL_FINISH_ERROR; the exception is kept in backend_errors)."""
+        from .sampling import mask_words, pack_mask
+        W = mask_words(vocab)
+
+        def _mask(_u, request, generated, n, out):
+            try:
+                a = np.asarray(mask_provider(int(request), np.ctypeslib.as_array(generated, shape=(n,)).copy() if n else np.empty(0, np.int32)))
+                w = pack_mask(a) if a.dtype == bool else np.asarray(a, dtype=np.uint32).reshape(-1)
+                if len(w) != W:
+                    raise ValueError("mask of %d words for a vocabulary of %d (%d words)" % (len(w), vocab, W))
+                np.ctypeslib.as_array(out, shape=(W,))[:] = w
+                return native.JL_OK
+            except Exception as e:  # noqa: BLE001 -- a Python exception must not unwind through the C caller
+                self.backend_errors.append(e)
+                return native.JL_ERR_INVALID
+
+        fn = native.SCHED_MASK_FN(_mask)
+        self._keep_mask = fn  # the C side keeps the pointer
+        self._check(self.lib.jl_sched_set_mask_provider(self.h, fn, None))
 
     @classmethod
     def over_backend(cls, reset_session, batch_forward, sample, decode, n_sessions, max_rows, max_context, prefill_tokens_per_step=0,
                      offload=None, restore=None, discard=None, forward_multi=None, sample_multi=None, decode_topkp=None,
                      sample_multi_topkp=None, decode_logprobs=None, sample_multi_logprobs=None, decode_penalized=None,
                      sample_multi_penalized=None, fork=None, retain=None, attach=None, release=None, retained=None, ctx_per_page=0,
-                     prefix_cache_pages=0):
+                     prefix_cache_pages=0, decode_constrained=None, sample_multi_constrained=None, vocab=0, mask_provider=None):
         """reset_session(session); batch_forward(session, tokens: np.int32[n], start_pos); sample(session, temperature, uniform) -> token;
         decode(sessions, tokens, positions: np.int32[n], temperatures, uniforms: np.float32[n]) -> next tokens; optionally the host-spill trio offload(session) -> handle,
         restore(session, handle), discard(handle).  Optionally the batched prompt pair (both or neither):
@@ -88,7 +129,10 @@ class SessionScheduler:
         take every call that holds a penalised request.  Optionally fork(src, positions, dst: np.int32[n]) gives the sessions dst the KV
         of src's positions [0, positions) and its last row; submit_n needs it for n > 1.  Optionally the prefix cache (all four with
         ctx_per_page, enabled when prefix_cache_pages > 0): retain(session, positions) -> handle, attach(handle, positions, session),
-        release(handle) and retained() -> (handles, pages held only by handles).
+        release(handle) and retained() -> (handles, pages held only by handles).  Optionally the constraint pair (both or neither, with the
+        vocabulary `vocab`): decode_constrained and sample_multi_constrained take the penalty pair's arguments plus a list of allowed
+        sets (one per row: None, or a bool[vocab]), return what the penalty pair returns and take every call that holds a constrained
+        request; mask_provider is the grammar engine of those requests (see _install_mask_provider).
         A raised exception fails the affected requests (JL_ERR_INVALID), exactly like a backend error code; a raised native.OutOfMemory
         returns JL_ERR_OOM."""
         self = cls.__new__(cls)
@@ -286,6 +330,32 @@ class SessionScheduler:
                                            native.SCHED_RETAINED_FN(_retained), int(ctx_per_page))
             self._keep_prefix = xb
             self._check(self.lib.jl_sched_set_prefix_cache(self.h, C.byref(xb), int(prefix_cache_pages)))
+        if (decode_constrained is None) != (sample_multi_constrained is None):
+            self.close()
+            raise ValueError("decode_constrained and sample_multi_constrained come together")
+        if decode_constrained is not None:
+            @guard
+            def _decode_constrained(_u, n, sessions, tokens, positions, temperatures, top_k, top_p, uniforms, top_n, pen, n_allow, allow,
+                                    allow_row, nxt, lp, ids, tlp):
+                arr = lambda p: np.ctypeslib.as_array(p, shape=(n,)).copy()  # noqa: E731
+                return put(n, decode_constrained(arr(sessions), arr(tokens), arr(positions), arr(temperatures), arr(top_k), arr(top_p),
+                                                 arr(uniforms), arr(top_n), penalty_rows(pen, n),
+                                                 allowed_rows(n_allow, allow, allow_row, n, vocab)), nxt, lp, ids, tlp)
+
+            @guard
+            def _sample_multi_constrained(_u, n, sessions, temperatures, top_k, top_p, uniforms, top_n, pen, n_allow, allow, allow_row, out,
+                                          lp, ids, tlp):
+                arr = lambda p: np.ctypeslib.as_array(p, shape=(n,)).copy()  # noqa: E731
+                return put(n, sample_multi_constrained(arr(sessions), arr(temperatures), arr(top_k), arr(top_p), arr(uniforms), arr(top_n),
+                                                       penalty_rows(pen, n), allowed_rows(n_allow, allow, allow_row, n, vocab)),
+                           out, lp, ids, tlp)
+
+            cb = native.SchedConstraintBackend(native.SCHED_DECODE_CONSTRAINED_FN(_decode_constrained),
+                                               native.SCHED_SAMPLE_MULTI_CONSTRAINED_FN(_sample_multi_constrained), int(vocab))
+            self._keep_constraints = cb
+            self._check(self.lib.jl_sched_set_constraint_backend(self.h, C.byref(cb)))
+        if mask_provider is not None:
+            self._install_mask_provider(mask_provider, int(vocab))
         return self
 
     def _check(self, rc):
@@ -293,18 +363,19 @@ class SessionScheduler:
             raise native.JlamaNativeError(rc, self.lib.jl_sched_last_error(self.h).decode())
 
     def submit(self, prompt, max_new, stop=(), keep_session=False, continue_request=-1, temperature=0.0, seed=0, top_k=0, top_p=1.0,
-               logprobs=-1, presence_penalty=0.0, frequency_penalty=0.0, repetition_penalty=1.0, logit_bias=None):
+               logprobs=-1, presence_penalty=0.0, frequency_penalty=0.0, repetition_penalty=1.0, logit_bias=None, constrained=False):
         """temperature 0 = arg-max; otherwise tokens are drawn from a uniform stream seeded with `seed`, with the reference's rule, or
         with the top-k / top-p rule (DESIGN §3.12) when top_k > 0 or top_p < 1.  logprobs >= 0: every generated token also gets its
         logprob and that many top alternatives (DESIGN §3.13), read with result_logprobs.  presence_penalty / frequency_penalty /
         repetition_penalty / logit_bias ({id: value}): every token is selected from its penalised logits (DESIGN §3.14), the history being
-        this request's prompt and generated tokens."""
+        this request's prompt and generated tokens.  constrained: every token is selected under the allowed set the mask provider
+        gives for it (DESIGN §3.18)."""
         from .model import _bias_pairs
         prompt = np.ascontiguousarray(prompt, dtype=np.int32)
         stop = np.ascontiguousarray(list(stop), dtype=np.int32)
         bi, bv = _bias_pairs(logit_bias)
         rid = self.lib.jl_sched_submit_penalized(self.h, native.ptr(prompt), len(prompt), max_new, native.ptr(stop) if len(stop) else None,
-                                                 len(stop), native.SCHED_KEEP_SESSION if keep_session else 0, continue_request,
+                                                 len(stop), _flags(keep_session, constrained), continue_request,
                                                  C.c_float(temperature), int(top_k), C.c_float(top_p), C.c_uint64(seed), int(logprobs),
                                                  C.c_float(presence_penalty), C.c_float(frequency_penalty), C.c_float(repetition_penalty),
                                                  len(bi), native.ptr(bi), native.ptr(bv))
@@ -313,7 +384,7 @@ class SessionScheduler:
         return rid
 
     def submit_n(self, prompt, n, max_new, stop=(), keep_session=False, continue_request=-1, temperature=0.0, seed=0, top_k=0, top_p=1.0,
-                 logprobs=-1, presence_penalty=0.0, frequency_penalty=0.0, repetition_penalty=1.0, logit_bias=None):
+                 logprobs=-1, presence_penalty=0.0, frequency_penalty=0.0, repetition_penalty=1.0, logit_bias=None, constrained=False):
         """n completions of one prompt (OpenAI's `n`) -> their request ids.  Member j is the request submit() makes with seed + j; the
         prompt is forwarded once and its KV pages are shared by the members (DESIGN §3.15)."""
         from .model import _bias_pairs
@@ -322,7 +393,7 @@ class SessionScheduler:
         bi, bv = _bias_pairs(logit_bias)
         ids = np.zeros(max(int(n), 1), dtype=np.int64)
         rc = self.lib.jl_sched_submit_n(self.h, int(n), native.ptr(prompt), len(prompt), max_new, native.ptr(stop) if len(stop) else None,
-                                        len(stop), native.SCHED_KEEP_SESSION if keep_session else 0, continue_request, C.c_float(temperature),
+                                        len(stop), _flags(keep_session, constrained), continue_request, C.c_float(temperature),
                                         int(top_k), C.c_float(top_p), C.c_uint64(seed), int(logprobs), C.c_float(presence_penalty),
                                         C.c_float(frequency_penalty), C.c_float(repetition_penalty), len(bi), native.ptr(bi), native.ptr(bv),
                                         native.ptr(ids))
