@@ -430,6 +430,14 @@ int jl_select_constrained(jl_ctx *ctx, int n, int vocab, const float *logits, in
  * of the replace-the-minimum top-k scan (MoEBlock.java:151-168) in the scan's order.  Refused (JL_ERR_INVALID) before any device work:
  * n < 1, n_experts outside 1..64, k outside 1..n_experts, a NULL pointer. */
 int jl_moe_route(jl_ctx *ctx, int n, int n_experts, int k, const float *logits, float *probs_out, int32_t *sel_out);
+/* The mixture-of-experts grouping kernel on HOST buffers, for crafted selections: sel [n][k] (experts in 0..n_experts-1) -> the
+ * pairs p = row * k + slot sorted by expert, a stable counting sort (ascending p within an expert): counts_out / offsets_out
+ * [n_experts] (the first place of each expert in pairs_out), pairs_out [n * k]; tiles_out [bound][4] {expert, first place, pairs, 0}
+ * cut each expert's list into runs of at most R pairs, expert by expert, *ntiles_out of them, with
+ * bound = (n * k + n_experts * (R - 1)) / R.  Refused (JL_ERR_INVALID) before any device work: n < 1, n_experts outside 1..64,
+ * k outside 1..min(8, n_experts), R outside 1..64, a selection out of range, a NULL pointer. */
+int jl_moe_group(jl_ctx *ctx, int n, int n_experts, int k, int R, const int32_t *sel, int32_t *counts_out, int32_t *offsets_out,
+                 int32_t *pairs_out, int32_t *tiles_out, int32_t *ntiles_out);
 /* AbstractModel.generate (:516-646) at temperature 0 over token ids: returns n_new tokens (the first is
  * sampled from the prompt's last row).  timings_ms (nullable double[2]) = {prompt, generate} wall ms like
  * Generator.Response.  logits_out HOST [n_new, vocab] or NULL. */

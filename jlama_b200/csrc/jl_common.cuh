@@ -132,6 +132,13 @@ struct GemvParams {
     void *wide_act;
     float *wide_part;
     unsigned *wide_cnt;
+    // grouped expert GEMM (jl_launch_gemm64_grouped): the tile table and pair list of jl_launch_moe_group; tile row r reads
+    // quantised row pair / g_div of wide_act (g_div = k: the token row of gate/up, 1: the pair's own h row for down_proj) and
+    // writes output row `pair`; the weights of segment i are w_tab[i][tile expert]
+    const int4 *g_tiles;
+    const int *g_ntiles;
+    const int *g_pairs;
+    int g_div;
 };
 __device__ __forceinline__ void gemv_seg_base(const GemvParams &p, int seg, const void *&w, const float *&ws) {
     if (p.sel) {
@@ -155,6 +162,12 @@ bool jl_gemm64_supported(const GemvParams &p, int prologue, int epilogue);
 int jl_launch_gemm64(jl_ctx *ctx, cudaStream_t stream, const GemvParams &p, int prologue, int epilogue);
 size_t jl_gemm64_act_bytes(int K);            // wide_act bytes for reduction length K
 size_t jl_gemm64_part_floats(int sm_count);   // wide_part floats
+// grouped expert GEMM: p.M activation rows quantised in a prologue launch, then one CTA per (tile, 128 weight rows) of the
+// first `tiles` entries of p.g_tiles (CTAs past *p.g_ntiles exit); tiles of at most jl_gemm64_group_rows(rows per expert) rows
+int jl_gemm64_group_rows(int max_rows_per_expert);
+bool jl_gemm64_grouped_supported(const GemvParams &p, int prologue, int epilogue, int R);
+int jl_launch_gemm64_grouped(jl_ctx *ctx, cudaStream_t stream, const GemvParams &p, int prologue, int epilogue, int R, int tiles);
+size_t jl_gemm64_q8_bytes(int rows, int K);   // quantised rows + block scales of the prologue
 
 // ---------------------------------------------------------------------------------------------
 // Element-wise / normalisation / sampling kernels (jl_elementwise.cu)
@@ -181,6 +194,17 @@ int jl_launch_activation(jl_ctx *ctx, cudaStream_t s, int type, float *x, int ro
 // MoE router: softmax over the expert logits of each row (VectorMath.softMax) + top-k by the reference's replace-the-minimum
 // scan (MoEBlock.java:151-168); sel[row * k + i] = i-th selected expert
 int jl_launch_moe_route(jl_ctx *ctx, cudaStream_t s, float *logits, int rows, int n_experts, int k, int32_t *sel);
+// MoE grouping of a step's rows by expert (one CTA): the pairs p = row * k + slot of sel [rows][k] by expert, a stable counting
+// sort (ascending p within an expert); counts / offsets [n_experts]; tiles {expert, first pair, pairs, 0} cut each expert's list
+// into runs of at most R, expert by expert; *ntiles = their number, at most jl_moe_tile_bound(rows * k, n_experts, R)
+struct MoeGroups {
+    int32_t *counts, *offsets, *pairs, *ntiles;
+    int4 *tiles;
+};
+static inline int jl_moe_tile_bound(int pairs, int n_experts, int R) { return (pairs + n_experts * (R - 1)) / R; }
+int jl_launch_moe_group(jl_ctx *ctx, cudaStream_t s, const int32_t *sel, int rows, int n_experts, int k, int R, const MoeGroups &g);
+// x[b] = (d[b k + k - 1] + ... + (d[b k + 1] + d[b k])) + xb[b], floats in slot order; d [rows * k][E]
+int jl_launch_moe_combine(jl_ctx *ctx, cudaStream_t s, const float *d, int rows, int k, int E, const float *xb, float *x);
 int jl_launch_softmax(jl_ctx *ctx, cudaStream_t s, float *x, int offset, int length);
 int jl_launch_silu_mul(jl_ctx *ctx, cudaStream_t s, float *gate, const float *up, int rows, int ld, int offset, int length);
 // fused producers of the BF16 operand of the tensor-core prefill GEMMs

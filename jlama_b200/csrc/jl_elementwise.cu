@@ -425,6 +425,126 @@ extern "C" int jl_moe_route(jl_ctx *ctx, int n, int n_experts, int k, const floa
     return JL_OK;
 }
 
+// ---- MoE grouping: a stable counting sort of a step's (row, slot) pairs by expert, and the tile table of the grouped expert GEMM --
+// One CTA of 1024 threads.  The scatter walks the pairs in chunks of 1024: a pair's place is its expert's running offset, plus the
+// pairs of that expert in earlier warps of the chunk, plus those in earlier lanes of its own warp (__match_any_sync), so the order
+// within an expert is the pair order whatever the warps' timing.
+#define MOE_GROUP_THREADS 1024
+__global__ void __launch_bounds__(MOE_GROUP_THREADS) moe_group_kernel(const int32_t *sel, int n, int n_experts, int R, MoeGroups g) {
+    __shared__ int cnt[64], run[64], tile0[65];
+    __shared__ int wc[MOE_GROUP_THREADS / 32][64];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid < 64) cnt[tid] = 0;
+    __syncthreads();
+    for (int i = tid; i < n; i += MOE_GROUP_THREADS) atomicAdd(&cnt[sel[i]], 1);
+    __syncthreads();
+    if (tid == 0) {
+        int o = 0, t = 0;
+        for (int e = 0; e < n_experts; e++) {
+            run[e] = o, tile0[e] = t;
+            o += cnt[e], t += (cnt[e] + R - 1) / R;
+        }
+        tile0[n_experts] = t;
+        *g.ntiles = t;
+    }
+    __syncthreads();
+    if (tid < n_experts) {
+        const int e = tid, c = cnt[e], o = run[e];
+        g.counts[e] = c, g.offsets[e] = o;
+        for (int f = 0, t = tile0[e]; f < c; f += R, t++) g.tiles[t] = make_int4(e, o + f, c - f < R ? c - f : R, 0);
+    }
+    for (int c0 = 0; c0 < n; c0 += MOE_GROUP_THREADS) {
+        const int i = c0 + tid;
+        const bool live = i < n;
+        const int e = live ? sel[i] : -1;
+        for (int j = tid; j < (MOE_GROUP_THREADS / 32) * 64; j += MOE_GROUP_THREADS) wc[j >> 6][j & 63] = 0;
+        __syncthreads();
+        const unsigned peers = __match_any_sync(0xffffffffu, e);
+        const int rank = __popc(peers & ((1u << lane) - 1u));
+        if (live && rank == 0) wc[warp][e] = __popc(peers);
+        __syncthreads();
+        if (tid < n_experts) { // the warps' counts -> their first places, warp by warp
+            int s = run[tid];
+            for (int w = 0; w < MOE_GROUP_THREADS / 32; w++) {
+                const int v = wc[w][tid];
+                wc[w][tid] = s, s += v;
+            }
+            run[tid] = s;
+        }
+        __syncthreads();
+        if (live) g.pairs[wc[warp][e] + rank] = i;
+        __syncthreads();
+    }
+}
+int jl_launch_moe_group(jl_ctx *ctx, cudaStream_t s, const int32_t *sel, int rows, int n_experts, int k, int R, const MoeGroups &g) {
+    if (rows < 1 || n_experts < 1 || n_experts > 64 || k < 1 || k > 8 || k > n_experts || R < 1)
+        return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "moe_group: %d rows, %d experts / top-%d, tiles of %d", rows, n_experts, k, R);
+    moe_group_kernel<<<1, MOE_GROUP_THREADS, 0, s>>>(sel, rows * k, n_experts, R, g);
+    ctx->launches++;
+    JL_CUDA_CHECK(ctx, cudaGetLastError());
+    return JL_OK;
+}
+
+// HOST-buffer entry point for crafted selections
+extern "C" int jl_moe_group(jl_ctx *ctx, int n, int n_experts, int k, int R, const int32_t *sel, int32_t *counts_out,
+                            int32_t *offsets_out, int32_t *pairs_out, int32_t *tiles_out, int32_t *ntiles_out) {
+    if (!ctx) return JL_ERR_INVALID;
+    if (n < 1 || n_experts < 1 || n_experts > 64 || k < 1 || k > 8 || k > n_experts || R < 1 || R > 64 || !sel || !counts_out ||
+        !offsets_out || !pairs_out || !tiles_out || !ntiles_out)
+        return jl_set_error(ctx, JL_ERR_INVALID, "moe_group: bad arguments (n=%d, experts=%d, k=%d, R=%d)", n, n_experts, k, R);
+    const size_t np = (size_t)n * k;
+    if (np > (size_t)1 << 24) return jl_set_error(ctx, JL_ERR_INVALID, "moe_group: %zu pairs", np);
+    for (size_t i = 0; i < np; i++)
+        if (sel[i] < 0 || sel[i] >= n_experts) return jl_set_error(ctx, JL_ERR_INVALID, "moe_group: selection %zu is %d", i, sel[i]);
+    std::lock_guard<std::mutex> lk(ctx->mu);
+    JL_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
+    const int bound = jl_moe_tile_bound((int)np, n_experts, R);
+    const size_t sb = np * 4, cb = (size_t)n_experts * 4, tb = (size_t)bound * sizeof(int4);
+    int32_t *ds = (int32_t *)jl_scratch(ctx, 0, sb);
+    char *dout = (char *)jl_scratch(ctx, 1, 2 * cb + sb + tb + 16);
+    if (!ds || !dout) return JL_ERR_OOM;
+    MoeGroups g;
+    g.tiles = (int4 *)dout, g.pairs = (int32_t *)(dout + tb), g.counts = (int32_t *)(dout + tb + sb);
+    g.offsets = g.counts + n_experts, g.ntiles = g.offsets + n_experts;
+    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(ds, sel, sb, cudaMemcpyHostToDevice, ctx->stream));
+    const int rc = jl_launch_moe_group(ctx, ctx->stream, ds, n, n_experts, k, R, g);
+    if (rc != JL_OK) return rc;
+    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(ntiles_out, g.ntiles, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(counts_out, g.counts, cb, cudaMemcpyDeviceToHost, ctx->stream));
+    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(offsets_out, g.offsets, cb, cudaMemcpyDeviceToHost, ctx->stream));
+    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(pairs_out, g.pairs, sb, cudaMemcpyDeviceToHost, ctx->stream));
+    JL_CUDA_CHECK(ctx, cudaStreamSynchronize(ctx->stream));
+    const int nt = *ntiles_out < bound ? *ntiles_out : bound;
+    JL_CUDA_CHECK(ctx, cudaMemcpy(tiles_out, g.tiles, (size_t)nt * sizeof(int4), cudaMemcpyDeviceToHost));
+    return JL_OK;
+}
+
+// ---- MoE combine: the expert outputs of each row summed in slot order, then the residual (the per-row loop's add chain) --------
+__global__ void moe_combine_kernel(const float4 *d, int rows, int k, int E4, const float4 *xb, float4 *x) {
+    const long long n = (long long)rows * E4;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const long long b = i / E4, c = i - b * E4;
+        float4 t = d[(size_t)b * k * E4 + c];
+        for (int s = 1; s < k; s++) {
+            const float4 v = d[((size_t)b * k + s) * E4 + c];
+            t = make_float4(__fadd_rn(v.x, t.x), __fadd_rn(v.y, t.y), __fadd_rn(v.z, t.z), __fadd_rn(v.w, t.w));
+        }
+        const float4 r = xb[i];
+        x[i] = make_float4(__fadd_rn(t.x, r.x), __fadd_rn(t.y, r.y), __fadd_rn(t.z, r.z), __fadd_rn(t.w, r.w));
+    }
+}
+int jl_launch_moe_combine(jl_ctx *ctx, cudaStream_t s, const float *d, int rows, int k, int E, const float *xb, float *x) {
+    if (rows <= 0) return JL_OK;
+    if (E % 4) return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "moe_combine: E=%d", E);
+    const long long n = (long long)rows * (E / 4);
+    long long blocks = (n + 255) / 256;
+    if (blocks > ctx->sm_count * 8) blocks = ctx->sm_count * 8;
+    moe_combine_kernel<<<(int)blocks, 256, 0, s>>>((const float4 *)d, rows, k, E / 4, (const float4 *)xb, (float4 *)x);
+    ctx->launches++;
+    JL_CUDA_CHECK(ctx, cudaGetLastError());
+    return JL_OK;
+}
+
 // ---- softmax (VectorMath.java:69-90), single row, one CTA ---------------------------------------------------------
 __global__ void softmax_kernel(float *x, int offset, int length) {
     __shared__ float red[32];

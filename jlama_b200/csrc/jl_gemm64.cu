@@ -17,6 +17,10 @@
 //   over `ks` CTAs; their partial tiles meet in a global workspace and the last CTA to arrive adds them in split order
 //   (deterministic: the same inputs give the same bits on every run).
 // Epilogues: store, residual add, SiLU(gate) * up -- as gemm8.
+// Grouped (mixture of experts, GR): the rows of one launch are the (row, slot) pairs of a step grouped by expert
+//   (jl_launch_moe_group); a CTA owns (tile, 128 weight rows of the tile's expert), gathers the tile's quantised rows and their
+//   block scales through the pair list, and writes each pair's output row.  No K split: a pair's bits are those of its own row
+//   against its expert, whatever the tile it lands in, its place there and the pairs that share the step.
 // lm_head (FA): F32 activations, not quantised (AbstractModel.java:444-449); the prologue splits each normalised value exactly into
 //   three BF16 planes and the block products run as bf16 x bf16 -> f32 MMAs against the weights as exact BF16 (see fa_chunk).
 #include "jl_common.cuh"
@@ -154,7 +158,11 @@ __global__ void __launch_bounds__(G64_THREADS) gemm64_quant_kernel(const GemvPar
 // FA (lm_head): F32 activations as three BF16 planes (gemm64_quant_kernel<*, true>), read by every warp straight from L2 / L1;
 // per block and plane two mma.sync.m16n8k16 (bf16 x bf16 -> f32) with the weights as exact BF16 (nibble - 8 or q), summed into one
 // f32 block sum, then acc = fmaf(sw, block sum, acc) in K order.
-template <int WDT, int EPI, int NT, bool FA>
+__device__ __forceinline__ void cp8(uint32_t dst, const void *src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::"r"(dst), "l"(src));
+}
+// GR: grid = tiles * groups, CTA (tile, group); ks == 1
+template <int WDT, int EPI, int NT, bool FA, bool GR = false>
 __global__ void __launch_bounds__(G64_THREADS, 1) gemm64_kernel(const GemvParams p, const int nst, const int ks) {
     extern __shared__ __align__(16) unsigned char smem[];
     constexpr int NW = EPI == EPI_SILU_MUL ? 2 : 1;
@@ -165,13 +173,27 @@ __global__ void __launch_bounds__(G64_THREADS, 1) gemm64_kernel(const GemvParams
     constexpr int MP = NT * 8; // padded rows
     constexpr int W_BYTES = G64_WARPS * NW * STRIP_STAGE, A_BYTES = FA ? 0 : MP * AST, S_BYTES = FA ? 0 : BPC * MP * 8;
     constexpr int STAGE = W_BYTES + A_BYTES + S_BYTES;
-    constexpr int UNROLL_U = NW * NT >= 12 ? 1 : BPC; // gate+up at 48 / 64 rows: 48 / 64 accumulators; a full unroll spills
+    // gate+up at 48 / 64 rows: 48 / 64 accumulators; a full unroll spills (grouped: from 32 rows, the gather's registers)
+    constexpr int UNROLL_U = NW * NT >= (GR ? 8 : 12) ? 1 : BPC;
     __shared__ int last_sh;
+    __shared__ int pair_sh[GR ? MP : 1], src_sh[GR ? MP : 1];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int g = lane >> 2, t = lane & 3;
-    const int K = p.K, nblk = K / 32, M = p.M;
-    const int grp = blockIdx.x / ks, split = blockIdx.x - grp * ks;
+    const int K = p.K, nblk = K / 32;
     const int strips = (p.total_rows + 15) / 16;
+    int grp = blockIdx.x / ks, split = blockIdx.x - grp * ks, M = p.M, expert = 0;
+    if (GR) {
+        const int groups = (strips + G64_WARPS - 1) / G64_WARPS, tile = blockIdx.x / groups;
+        if (tile >= *p.g_ntiles) return;
+        grp = blockIdx.x - tile * groups, split = 0;
+        const int4 tl = p.g_tiles[tile];
+        expert = tl.x, M = tl.z;
+        if (tid < MP) {
+            const int pr = p.g_pairs[tl.y + (tid < M ? tid : 0)]; // padding rows repeat the first pair; never stored
+            pair_sh[tid] = pr, src_sh[tid] = pr / p.g_div;
+        }
+        __syncthreads();
+    }
     const int strip = grp * G64_WARPS + warp;
     const bool have = strip < strips;
     const int cpk = nblk / BPC / ks; // chunks of this CTA
@@ -193,7 +215,8 @@ __global__ void __launch_bounds__(G64_THREADS, 1) gemm64_kernel(const GemvParams
                 if (p.nseg > 2 && local >= p.seg[1].rows) local -= p.seg[1].rows, seg = 2;
             }
         }
-        gemv_seg_base(p, seg, wb[w], wsb[w]);
+        if (GR) wb[w] = p.w_tab[seg][expert], wsb[w] = p.ws_tab[seg][expert];
+        else gemv_seg_base(p, seg, wb[w], wsb[w]);
         local0[w] = local;
     }
     const int rows_left = p.total_rows - strip * 16;
@@ -201,7 +224,7 @@ __global__ void __launch_bounds__(G64_THREADS, 1) gemm64_kernel(const GemvParams
     const unsigned long long pol = l2_evict_first_policy();
     const uint32_t smem_u32 = (uint32_t)__cvta_generic_to_shared(smem);
     const int8_t *act = (const int8_t *)p.wide_act;
-    const unsigned char *act_s = (const unsigned char *)p.wide_act + (size_t)MP * K;
+    const unsigned char *act_s = (const unsigned char *)p.wide_act + (size_t)(GR ? p.M : MP) * K; // GR: p.M quantised rows
 
     auto issue = [&](int q) {
         if (q < cpk) {
@@ -221,10 +244,16 @@ __global__ void __launch_bounds__(G64_THREADS, 1) gemm64_kernel(const GemvParams
             const uint32_t as = st + W_BYTES;
             for (int i = tid; i < MP * (KC / 16); i += G64_THREADS) {
                 const int r = i / (KC / 16), o = (i - r * (KC / 16)) * 16;
-                cp16(as + r * AST + o, act + (size_t)r * K + (size_t)c * KC + o);
+                cp16(as + r * AST + o, act + (size_t)(GR ? src_sh[r] : r) * K + (size_t)c * KC + o);
             }
             const uint32_t ss = as + A_BYTES;
-            for (int i = tid; i < S_BYTES / 16; i += G64_THREADS) cp16(ss + i * 16, act_s + (size_t)c * S_BYTES + (size_t)i * 16);
+            if (GR) // the {scale, offset} of each gathered row, block by block: [BPC][MP] as the staged layout
+                for (int i = tid; i < BPC * MP; i += G64_THREADS) {
+                    const int u = i / MP, r = i - u * MP;
+                    cp8(ss + i * 8, act_s + ((size_t)(c * BPC + u) * p.M + src_sh[r]) * 8);
+                }
+            else
+                for (int i = tid; i < S_BYTES / 16; i += G64_THREADS) cp16(ss + i * 16, act_s + (size_t)c * S_BYTES + (size_t)i * 16);
         }
         cp_commit();
     };
@@ -380,10 +409,11 @@ __global__ void __launch_bounds__(G64_THREADS, 1) gemm64_kernel(const GemvParams
                 for (int jj = 0; jj < 2; jj++) {
                     const int m = 8 * j + 2 * t + jj;
                     if (m >= M) continue;
+                    const int o = GR ? pair_sh[m] : m;
                     float v = acc[NW - 1][j][2 * h + jj];
-                    if (EPI == EPI_ADD_RESIDUAL) v = __fadd_rn(v, p.residual[(size_t)m * p.res_ld + (p.row0 + local)]);
+                    if (EPI == EPI_ADD_RESIDUAL) v = __fadd_rn(v, p.residual[(size_t)o * p.res_ld + (p.row0 + local)]);
                     if (EPI == EPI_SILU_MUL) v = __fmul_rn(silu_ref(acc[0][j][2 * h + jj]), v);
-                    sg.out[(size_t)m * sg.out_ld + p.row0 + local + sg.out_off] = v;
+                    sg.out[(size_t)o * sg.out_ld + p.row0 + local + sg.out_off] = v;
                 }
         }
     }
@@ -408,11 +438,9 @@ static int g64_stages(int wdt, int epi, int nt, bool fa) {
 size_t jl_gemm64_act_bytes(int K) { return (size_t)3 * JL_MAX_DECODE_ROWS * K * 2; }
 size_t jl_gemm64_part_floats(int sm_count) { return (size_t)sm_count * 2 * 8 * 4 * G64_THREADS; }
 
-// usable for this launch?  9..64 rows, Q4 / Q8_0 weights, whole 128-byte chunks; Q8 activations made in the prologue, or F32
-// activations (store epilogue, one tensor: the lm_head) split into BF16 planes in the prologue
-bool jl_gemm64_supported(const GemvParams &p, int prologue, int epilogue) {
-    if (p.M <= GEMV_MAX_M || p.M > JL_MAX_DECODE_ROWS || p.sel) return false;
-    if (!p.wide_act || !p.wide_part || !p.wide_cnt) return false;
+// the weight shape, prologue and epilogue of a launch at NT row tiles: Q4 / Q8_0 weights, whole 128-byte chunks; Q8 activations
+// made in the prologue, or F32 activations (store epilogue, one tensor: the lm_head) split into BF16 planes in the prologue
+static bool g64_shape_ok(const GemvParams &p, int prologue, int epilogue, int nt) {
     if (p.w_dtype != JL_Q4 && p.w_dtype != JL_I8) return false;
     const bool fa = g64_fa(prologue);
     if (prologue != PRO_F32_QUANT && prologue != PRO_RMSNORM_QUANT && !fa) return false;
@@ -426,7 +454,26 @@ bool jl_gemm64_supported(const GemvParams &p, int prologue, int epilogue) {
     if (epilogue != EPI_SILU_MUL)
         for (int i = 0; i + 1 < p.nseg; i++)
             if (p.seg[i].rows % 16) return false; // a strip must not straddle two weight tensors
-    return g64_stages(p.w_dtype, epilogue, g64_nt(p.M), fa) >= 2;
+    return g64_stages(p.w_dtype, epilogue, nt, fa) >= 2;
+}
+
+// usable for this launch?  9..64 rows
+bool jl_gemm64_supported(const GemvParams &p, int prologue, int epilogue) {
+    if (p.M <= GEMV_MAX_M || p.M > JL_MAX_DECODE_ROWS || p.sel) return false;
+    if (!p.wide_act || !p.wide_part || !p.wide_cnt) return false;
+    return g64_shape_ok(p, prologue, epilogue, g64_nt(p.M));
+}
+
+// grouped: tiles of R = 16, 32, 48 or 64 rows (NT = R / 8), the smallest that holds every pair of an expert when no expert can
+// receive more than max_rows_per_expert (a step's rows: top-k selects distinct experts), 64 past that
+int jl_gemm64_group_rows(int max_rows_per_expert) { return 8 * g64_nt(max_rows_per_expert); }
+size_t jl_gemm64_q8_bytes(int rows, int K) { return (size_t)rows * K + (size_t)rows * (K / 32) * 8; }
+bool jl_gemm64_grouped_supported(const GemvParams &p, int prologue, int epilogue, int R) {
+    if (R != 8 * g64_nt(R) || p.M < 1 || p.sel || !p.wide_act || !p.g_tiles || !p.g_ntiles || !p.g_pairs || p.g_div < 1) return false;
+    if (!p.w_tab[0] || !p.ws_tab[0] || (epilogue == EPI_SILU_MUL && (!p.w_tab[1] || !p.ws_tab[1]))) return false;
+    if (prologue != PRO_F32_QUANT && prologue != PRO_RMSNORM_QUANT) return false;
+    if (epilogue == EPI_ADD_RESIDUAL) return false; // a pair's output row is not a residual row
+    return g64_shape_ok(p, prologue, epilogue, R / 8);
 }
 
 // K splits: the smallest power of two (<= 8, dividing the chunk count) whose CTAs cover the SMs, and no more CTAs than SMs
@@ -438,40 +485,43 @@ static int g64_ksplit(const GemvParams &p, int sm_count) {
     return ks;
 }
 
-template <int WDT, int EPI, int NT, bool FA>
-static int launch_g64(jl_ctx *ctx, cudaStream_t stream, const GemvParams &p) {
-    auto kern = gemm64_kernel<WDT, EPI, NT, FA>;
+// tiles > 0: grouped, one CTA per (tile, group) and no K split
+template <int WDT, int EPI, int NT, bool FA, bool GR>
+static int launch_g64(jl_ctx *ctx, cudaStream_t stream, const GemvParams &p, int tiles) {
+    auto kern = gemm64_kernel<WDT, EPI, NT, FA, GR>;
     const int nst = g64_stages(WDT, EPI, NT, FA);
     const size_t smem = (size_t)nst * g64_stage(WDT, EPI, NT, FA);
     static size_t configured[JL_MAX_DEVICES] = {};
     JL_CUDA_CHECK(ctx, jl_ensure_dyn_smem(kern, ctx->device, smem, configured));
     const int groups = ((p.total_rows + 15) / 16 + G64_WARPS - 1) / G64_WARPS;
-    const int ks = g64_ksplit(p, ctx->sm_count);
-    JL_CUDA_CHECK(ctx, jl_launch_kernel(kern, dim3(groups * ks), dim3(G64_THREADS), smem, stream, p, nst, ks));
+    const int ks = GR ? 1 : g64_ksplit(p, ctx->sm_count);
+    JL_CUDA_CHECK(ctx, jl_launch_kernel(kern, dim3(groups * (GR ? tiles : ks)), dim3(G64_THREADS), smem, stream, p, nst, ks));
     ctx->launches++;
     return JL_OK;
 }
-template <int WDT, int EPI, bool FA>
-static int launch_g64_n(jl_ctx *ctx, cudaStream_t stream, const GemvParams &p) {
-    switch (g64_nt(p.M)) {
-        case 2: return launch_g64<WDT, EPI, 2, FA>(ctx, stream, p);
-        case 4: return launch_g64<WDT, EPI, 4, FA>(ctx, stream, p);
-        case 6: return launch_g64<WDT, EPI, 6, FA>(ctx, stream, p);
-        default: return launch_g64<WDT, EPI, 8, FA>(ctx, stream, p);
+template <int WDT, int EPI, bool FA, bool GR = false>
+static int launch_g64_n(jl_ctx *ctx, cudaStream_t stream, const GemvParams &p, int nt, int tiles = 0) {
+    switch (nt) {
+        case 2: return launch_g64<WDT, EPI, 2, FA, GR>(ctx, stream, p, tiles);
+        case 4: return launch_g64<WDT, EPI, 4, FA, GR>(ctx, stream, p, tiles);
+        case 6: return launch_g64<WDT, EPI, 6, FA, GR>(ctx, stream, p, tiles);
+        default: return launch_g64<WDT, EPI, 8, FA, GR>(ctx, stream, p, tiles);
     }
 }
 template <int WDT>
 static int launch_g64_e(jl_ctx *ctx, cudaStream_t stream, const GemvParams &p, int prologue, int epilogue) {
-    if (g64_fa(prologue)) return launch_g64_n<WDT, EPI_STORE, true>(ctx, stream, p);
+    const int nt = g64_nt(p.M);
+    if (g64_fa(prologue)) return launch_g64_n<WDT, EPI_STORE, true>(ctx, stream, p, nt);
     switch (epilogue) {
-        case EPI_STORE: return launch_g64_n<WDT, EPI_STORE, false>(ctx, stream, p);
-        case EPI_ADD_RESIDUAL: return launch_g64_n<WDT, EPI_ADD_RESIDUAL, false>(ctx, stream, p);
-        default: return launch_g64_n<WDT, EPI_SILU_MUL, false>(ctx, stream, p);
+        case EPI_STORE: return launch_g64_n<WDT, EPI_STORE, false>(ctx, stream, p, nt);
+        case EPI_ADD_RESIDUAL: return launch_g64_n<WDT, EPI_ADD_RESIDUAL, false>(ctx, stream, p, nt);
+        default: return launch_g64_n<WDT, EPI_SILU_MUL, false>(ctx, stream, p, nt);
     }
 }
 
-int jl_launch_gemm64(jl_ctx *ctx, cudaStream_t stream, const GemvParams &p, int prologue, int epilogue) {
-    const int mpad = g64_nt(p.M) * 8, q4 = p.w_dtype == JL_Q4 ? 1 : 0;
+// the prologue of mpad rows into p.wide_act
+static int g64_prologue(jl_ctx *ctx, cudaStream_t stream, const GemvParams &p, int prologue, int mpad) {
+    const int q4 = p.w_dtype == JL_Q4 ? 1 : 0;
     cudaError_t e;
     switch (prologue) {
         case PRO_RMSNORM_QUANT: e = jl_launch_kernel(gemm64_quant_kernel<true, false>, dim3(mpad), dim3(G64_THREADS), 0, stream, p, mpad, q4); break;
@@ -481,5 +531,29 @@ int jl_launch_gemm64(jl_ctx *ctx, cudaStream_t stream, const GemvParams &p, int 
     }
     JL_CUDA_CHECK(ctx, e);
     ctx->launches++;
+    return JL_OK;
+}
+
+int jl_launch_gemm64(jl_ctx *ctx, cudaStream_t stream, const GemvParams &p, int prologue, int epilogue) {
+    const int rc = g64_prologue(ctx, stream, p, prologue, g64_nt(p.M) * 8);
+    if (rc != JL_OK) return rc;
     return p.w_dtype == JL_Q4 ? launch_g64_e<JL_Q4>(ctx, stream, p, prologue, epilogue) : launch_g64_e<JL_I8>(ctx, stream, p, prologue, epilogue);
+}
+
+template <int WDT>
+static int launch_g64_grouped(jl_ctx *ctx, cudaStream_t stream, const GemvParams &p, int epilogue, int nt, int tiles) {
+    if (epilogue == EPI_SILU_MUL) return launch_g64_n<WDT, EPI_SILU_MUL, false, true>(ctx, stream, p, nt, tiles);
+    return launch_g64_n<WDT, EPI_STORE, false, true>(ctx, stream, p, nt, tiles);
+}
+
+// the p.M rows of p.a quantised once (the prologue of jl_launch_gemm64), then the grouped GEMM over `tiles` tile entries
+int jl_launch_gemm64_grouped(jl_ctx *ctx, cudaStream_t stream, const GemvParams &p_in, int prologue, int epilogue, int R, int tiles) {
+    if (!jl_gemm64_grouped_supported(p_in, prologue, epilogue, R)) return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "gemm64 grouped: launch not supported");
+    if (tiles < 1) return JL_OK;
+    GemvParams p = p_in;
+    p.trace = nullptr, p.norm_inv_E = p.norm_E > 0 ? 1.0 / (double)p.norm_E : 0.0;
+    const int rc = g64_prologue(ctx, stream, p, prologue, p.M);
+    if (rc != JL_OK) return rc;
+    return p.w_dtype == JL_Q4 ? launch_g64_grouped<JL_Q4>(ctx, stream, p, epilogue, R / 8, tiles)
+                              : launch_g64_grouped<JL_I8>(ctx, stream, p, epilogue, R / 8, tiles);
 }

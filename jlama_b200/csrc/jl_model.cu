@@ -116,6 +116,11 @@ struct jl_model {
     float **moe_stab = nullptr;      // device [layers][3][n_exp] scale pointers
     float *moe_logits = nullptr;     // [maxB][n_exp]
     int32_t *moe_sel = nullptr;      // [maxB][exp_k]
+    // grouped expert GEMMs (forward_rows, M >= 2): Q8 rows of xb (gate/up) and of h (down_proj), each pair's down_proj output
+    // [maxB * exp_k][E], and the grouping of jl_launch_moe_group (one allocation, moe_grp.tiles first)
+    void *moe_qa = nullptr, *moe_qh = nullptr;
+    float *moe_dout = nullptr;
+    MoeGroups moe_grp = {};
     // persistent decode kernel (jl_pdecode.cu)
     bool pd_ok = false;
     int pd_wdtype = JL_Q4;
@@ -513,6 +518,16 @@ extern "C" int jl_model_finalize(jl_model *m) {
         M_CHECK(dev_alloc(ctx, (void **)&m->moe_stab, ne * sizeof(float *)));
         JL_CUDA_CHECK(ctx, cudaMemcpy(m->moe_wtab, wt.data(), ne * sizeof(void *), cudaMemcpyHostToDevice));
         JL_CUDA_CHECK(ctx, cudaMemcpy(m->moe_stab, st.data(), ne * sizeof(float *), cudaMemcpyHostToDevice));
+        // grouped expert GEMMs: at most maxB * k + n_exp tiles for any tile height
+        const size_t H = c.hidden_length, P = B * m->exp_k, T = P + m->n_exp;
+        M_CHECK(dev_alloc(ctx, &m->moe_qa, jl_gemm64_q8_bytes((int)B, E)));
+        M_CHECK(dev_alloc(ctx, &m->moe_qh, jl_gemm64_q8_bytes((int)P, (int)H)));
+        M_CHECK(dev_alloc(ctx, (void **)&m->moe_dout, P * E * 4));
+        char *gb = nullptr;
+        M_CHECK(dev_alloc(ctx, (void **)&gb, T * sizeof(int4) + (P + 2 * (size_t)m->n_exp + 1) * 4));
+        m->moe_grp.tiles = (int4 *)gb, m->moe_grp.pairs = (int32_t *)(gb + T * sizeof(int4));
+        m->moe_grp.counts = m->moe_grp.pairs + P, m->moe_grp.offsets = m->moe_grp.counts + m->n_exp;
+        m->moe_grp.ntiles = m->moe_grp.offsets + m->n_exp;
     }
     M_CHECK(dev_alloc(ctx, (void **)&m->partial, B * E * 4));
     if (c.arch == JL_ARCH_GPT2) M_CHECK(dev_alloc(ctx, (void **)&m->ln, B * E * 4)); // LayerNorm output (its own tensor in the reference too)
@@ -736,7 +751,7 @@ extern "C" int jl_model_free(jl_model *m) {
             if (!drop_ref(m, p)) cudaFree(p);
     void *bufs[] = {m->d_copy_tab,m->ln, m->hbuf2, m->abf, m->rope, m->page_table_dev, m->x, m->xb, m->q, m->k, m->v, m->att, m->hbuf, m->partial, m->logits,
                     m->last_hidden, m->attn_ws, m->d_tokens, m->d_positions, m->d_sessions, m->d_next, m->d_hist, m->d_counter,
-                    m->argmax_scratch, m->fda_done, m->moe_wtab, m->moe_stab, m->moe_logits, m->moe_sel, m->pd_sync, m->pd_slots, m->pd_att_done, m->pd_trace, m->ll_o, m->ll_d, m->ll_a, m->wide_act, m->wide_part, m->wide_cnt, m->d_pa_tab, m->d_rows, m->topkp_ex, m->d_topkp,
+                    m->argmax_scratch, m->fda_done, m->moe_wtab, m->moe_stab, m->moe_logits, m->moe_sel, m->moe_qa, m->moe_qh, m->moe_dout, m->moe_grp.tiles, m->pd_sync, m->pd_slots, m->pd_att_done, m->pd_trace, m->ll_o, m->ll_d, m->ll_a, m->wide_act, m->wide_part, m->wide_cnt, m->d_pa_tab, m->d_rows, m->topkp_ex, m->d_topkp,
                     m->score_logits, m->pen_out, m->pen_bias, m->pen_cnt, m->d_pen_tab, m->d_mask};
     for (void *p : bufs)
         if (p) cudaFree(p);
@@ -975,7 +990,7 @@ static int forward_rows(jl_model *m, int M, int splits, bool distinct_sessions =
             }
         }
         if (m->n_exp > 0) {
-            // ---- mixture of experts (MoEBlock.java:73-149), one row at a time: router GEMV -> softmax + top-k on the device ->
+            // ---- mixture of experts (MoEBlock.java:73-149); the grouped path below, else one row at a time: router GEMV -> softmax + top-k on the device ->
             // per selected expert gate/up (SiLU*up fused) and down_proj through the expert pointer tables; the expert results
             // are summed UNWEIGHTED in selection order (:139-143), then the residual is added (TransformerBlock.java:203).
             // Row b of the result is the sum over row b's experts (the reference's copy of expert 0's result into row 0 for
@@ -988,6 +1003,35 @@ static int forward_rows(jl_model *m, int M, int splits, bool distinct_sessions =
             float **st = m->moe_stab + (size_t)L * 3 * NE;
             const size_t own = ((size_t)L * NE + c.tp_rank) * 3; // first expert held by this rank: shapes / dtype of every expert
             const bool aq = act_q(m->moe_w[own]);
+            // grouped (M >= 2, Q8 activations, one rank): the router over all M rows, the rows grouped by expert on the device,
+            // and each selected expert streamed once per launch for all of its rows (jl_launch_gemm64_grouped); a fixed number
+            // of launches whatever M is, sized from the tile bound because the selections are only known on the device
+            const int R = jl_gemm64_group_rows(M);
+            GemvParams gu = gemv_params(m->moe_w[own], m->hbuf, H, m->xb, E, H), dn = gemv_params(m->moe_w[own + 1], m->moe_dout, E, m->hbuf, H, E);
+            {
+                gu.nseg = 2; // output rows: pair b * k + i of hbuf / moe_dout
+                set_w(gu, 1, m->moe_w[own], m->hbuf, H);
+                gu.w_tab[0] = (const void *const *)(wt + 0 * NE), gu.ws_tab[0] = (const float *const *)(st + 0 * NE); // w1
+                gu.w_tab[1] = (const void *const *)(wt + 2 * NE), gu.ws_tab[1] = (const float *const *)(st + 2 * NE); // w3
+                set_norm(gu, lw[JL_L_FFN_NORM], m);
+                gu.M = M, gu.wide_act = m->moe_qa, gu.g_div = KE;
+                dn.w_tab[0] = (const void *const *)(wt + 1 * NE), dn.ws_tab[0] = (const float *const *)(st + 1 * NE); // w2
+                dn.M = M * KE, dn.wide_act = m->moe_qh, dn.g_div = 1;
+                for (GemvParams *q : {&gu, &dn}) q->g_tiles = m->moe_grp.tiles, q->g_ntiles = m->moe_grp.ntiles, q->g_pairs = m->moe_grp.pairs;
+            }
+            if (M >= 2 && aq && c.tp_size == 1 && jl_gemm64_grouped_supported(gu, PRO_RMSNORM_QUANT, EPI_SILU_MUL, R) &&
+                jl_gemm64_grouped_supported(dn, PRO_F32_QUANT, EPI_STORE, R)) {
+                GemvParams p = gemv_params(m->moe_gate[L], m->moe_logits, NE, m->xb, E, NE);
+                set_norm(p, lw[JL_L_FFN_NORM], m);
+                M_CHECK(run_gemm(m, p, act_q(m->moe_gate[L]) ? PRO_RMSNORM_QUANT : PRO_RMSNORM_F32, EPI_STORE, M, distinct_sessions));
+                M_CHECK(jl_launch_moe_route(ctx, m->stream, m->moe_logits, M, NE, KE, m->moe_sel));
+                M_CHECK(jl_launch_moe_group(ctx, m->stream, m->moe_sel, M, NE, KE, R, m->moe_grp));
+                const int tiles = jl_moe_tile_bound(M * KE, NE, R);
+                M_CHECK(jl_launch_gemm64_grouped(ctx, m->stream, gu, PRO_RMSNORM_QUANT, EPI_SILU_MUL, R, tiles));
+                M_CHECK(jl_launch_gemm64_grouped(ctx, m->stream, dn, PRO_F32_QUANT, EPI_STORE, R, tiles));
+                M_CHECK(jl_launch_moe_combine(ctx, m->stream, m->moe_dout, M, KE, E, m->xb, m->x));
+                continue;
+            }
             for (int b = 0; b < M; b++) {
                 {
                     GemvParams p = gemv_params(m->moe_gate[L], m->moe_logits + (size_t)b * NE, NE, m->xb + (size_t)b * E, E, NE);

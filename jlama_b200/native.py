@@ -269,6 +269,7 @@ SIGNATURES = {
     "jl_model_sample_multi_constrained": (_i, [_vp, _i] + [_vp] * 7 + [_i] + [_vp] * 7),
     "jl_select_constrained": (_i, [_vp, _i, _i, _vp, _i64] + [_vp] * 5 + [_i] + [_vp] * 3),
     "jl_moe_route": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),
+    "jl_moe_group": (_i, [_vp, _i, _i, _i, _i] + [_vp] * 6),
     "jl_model_decode_resident": (_i, [_vp, _i, C.c_int32, _i, _i, _vp]),
     "jl_model_read_kv": (_i, [_vp, _i, _i, _i, _i, _vp]),
     "jl_model_kv_save": (_i, [_vp, _i, C.c_char_p, C.c_char_p]),
