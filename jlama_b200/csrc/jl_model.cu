@@ -2658,13 +2658,17 @@ extern "C" int jl_model_debug_read(jl_model *m, int which, float *out, int64_t n
     std::lock_guard<std::recursive_mutex> model_lock(m->mu);
     jl_ctx *ctx = m->ctx;
     JL_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
-    // 8 / 9: the router probabilities (the route kernel overwrites the logits) and the selections (int32 bits) of MoE models
-    const float *src[10] = {m->x, m->xb, m->q, m->k, m->v, m->att, m->hbuf, m->logits, m->moe_logits, (const float *)m->moe_sel};
+    // 8 / 9: the router probabilities (the route kernel overwrites the logits) and the selections (int32 bits) of MoE models;
+    // 10 / 11: the up projection and the BF16 operand buffer (uint16 pairs per word) of tensor-core prefill models
+    const float *src[12] = {m->x, m->xb, m->q, m->k, m->v, m->att, m->hbuf, m->logits, m->moe_logits, (const float *)m->moe_sel, m->hbuf2,
+                            (const float *)m->abf};
     const size_t B = m->maxB;
-    const size_t cap[10] = {B * m->cfg.embedding_length, B * m->cfg.embedding_length, B * m->attn_seg, B * m->kv_seg, B * m->kv_seg,
+    size_t kmax = m->cfg.embedding_length > m->h_seg ? m->cfg.embedding_length : m->h_seg;
+    if ((size_t)m->attn_seg > kmax) kmax = m->attn_seg;
+    const size_t cap[12] = {B * m->cfg.embedding_length, B * m->cfg.embedding_length, B * m->attn_seg, B * m->kv_seg, B * m->kv_seg,
                             B * m->attn_seg, B * (m->n_exp > 0 ? (size_t)m->exp_k * m->cfg.hidden_length : m->h_seg),
-                            (size_t)m->cfg.max_sessions * m->cfg.vocab_size, B * m->n_exp, B * m->exp_k};
-    if (which < 0 || which > 9 || (size_t)n > cap[which] || !src[which])
+                            (size_t)m->cfg.max_sessions * m->cfg.vocab_size, B * m->n_exp, B * m->exp_k, B * m->h_seg, B * kmax / 2};
+    if (which < 0 || which > 11 || (size_t)n > cap[which] || !src[which])
         return jl_set_error(ctx, JL_ERR_INVALID, "debug_read: bad buffer / size");
     JL_CUDA_CHECK(ctx, cudaStreamSynchronize(m->stream));
     JL_CUDA_CHECK(ctx, cudaMemcpy(out, src[which], (size_t)n * 4, cudaMemcpyDeviceToHost));

@@ -526,7 +526,10 @@ class LlamaModel:
     def debug_read(self, which, n):
         """Test hook: internal activation buffer of the last forward/decode call (0 x, 1 xb, 2 q, 3 k, 4 v, 5 att, 6 h, 7 logits).
         Mixture-of-experts models: h holds one row per (row, selected expert), expert i of row b at row b * experts_per_token + i;
-        8 is the router probabilities [rows, experts] and 9 the selected experts [rows, experts_per_token] (int32 bits: .view(np.int32))."""
+        8 is the router probabilities [rows, experts] and 9 the selected experts [rows, experts_per_token] (int32 bits: .view(np.int32)).
+        Tensor-core prefill models (prefill_tensor_core=1): 10 is the up projection [rows, H] (h holds the gate projection there),
+        and 11 the BF16 operand buffer of the last GEMM, n float words of two BF16 each (.view(np.uint16)); after a tensor-core pass
+        it holds bf16(silu(gate) * up) of the last layer [rows, H], down_proj's input.  Other models refuse 10 and 11."""
         out = np.empty(n, dtype=np.float32)
         self.ctx.check(self.lib.jl_model_debug_read(self.h, which, ptr(out), n))
         return out

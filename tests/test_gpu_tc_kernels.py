@@ -90,10 +90,12 @@ def gemm_err_blocked(c, a16, wdt, q, s, tau=GEMM_TAU, block=2048):
     return worst, level
 
 
-def attn_emulated(q, k, v, pos0, group, scale, causal_shift=0, head_map=None, skip_rescale_tile=None):
+def attn_emulated(q, k, v, pos0, group, scale, causal_shift=0, head_map=None, skip_rescale_tile=None, ambiguity=False):
     """Prefill attention of rows at positions pos0 .. pos0 + R - 1 with the kernel's rounding points.  q [R, Hq, hs], k / v
     [P, Hkv, hs] (positions 0 .. P - 1) as float32; returns [R, Hq, hs] float64.  The keyword arguments mutate the computation
-    (the sharpness tests): the causal limit moved, query heads mapped to other KV heads, the rescale skipped on one tile."""
+    (the sharpness tests): the causal limit moved, query heads mapped to other KV heads, the rescale skipped on one tile.
+    ambiguity: also return the allowance [R, Hq, hs] for elements of P whose BF16 rounding the kernel's f32 scores can move: e
+    within 2^-20 scale sum|q k| + 2^-23 (|s| + |max|) + 2^-21 (relative) of a BF16 midpoint adds one BF16 step * |V| / l."""
     R, Hq, hs = q.shape
     P = k.shape[0]
     kv_of = np.arange(Hq) // group if head_map is None else np.asarray(head_map)
@@ -104,6 +106,7 @@ def attn_emulated(q, k, v, pos0, group, scale, causal_shift=0, head_map=None, sk
     m = np.full((R, Hq), -np.inf)
     l = np.zeros((R, Hq))
     o = np.zeros((R, Hq, hs))
+    amb = np.zeros((R, Hq, hs))
     with np.errstate(invalid="ignore", over="ignore"):
         for tile, t0 in enumerate(range(0, int(lim.max()) + 1, 64)):
             kt, vt = kb[t0:t0 + 64], vb[t0:t0 + 64]
@@ -117,7 +120,16 @@ def attn_emulated(q, k, v, pos0, group, scale, causal_shift=0, head_map=None, sk
             e = np.exp(s - mx[..., None])
             l = l * al + e.sum(axis=-1)
             o = o * al[..., None] + np.einsum("rhk,khd->rhd", bf16(e).astype(np.float64), vt)
+            if ambiguity:
+                lo = T.bfloat16_to_float32((e.astype(np.float32).view(np.uint32) >> 16).astype(np.uint16)).astype(np.float64)
+                step = np.ldexp(1.0, np.frexp(lo)[1] - 8)  # the BF16 step above lo
+                nat = np.einsum("rhd,khd->rhk", np.abs(qb), np.abs(kt)) * scale
+                win = 2.0 ** -20 * nat + 2.0 ** -23 * (np.abs(s) + np.abs(mx)[..., None]) + 2.0 ** -21
+                near = vis[:, None, :] & (np.abs(e - (lo + 0.5 * step)) <= win * e)
+                amb = amb * al[..., None] + np.einsum("rhk,khd->rhd", np.where(near, step, 0.0), np.abs(vt))
             m = mx
+    if ambiguity:
+        return o / l[..., None], amb / l[..., None]
     return o / l[..., None]
 
 
