@@ -260,7 +260,8 @@ int jl_model_set_tensor(jl_model *m, int layer, int slot, int64_t tensor_id);
 int jl_model_set_expert_tensor(jl_model *m, int layer, int expert, int which, int64_t tensor_id);
 /* GPT-2 family: bias vectors ([1, n] F32/BF16) and the position-embedding table, see JL_AUX_* */
 int jl_model_set_aux_tensor(jl_model *m, int layer, int which, int64_t tensor_id);
-/* allocate scratch + KV page pool, build RoPE table, capture graphs */
+/* allocate scratch + KV page pool, build RoPE table, capture graphs.  JL_ERR_UNSUPPORTED for weights no kernel runs: F32 / BF16
+ * gate/up of a Llama model or F32 / BF16 experts (their SiLU * up epilogue is implemented for Q4 / I8 weights only). */
 int jl_model_finalize(jl_model *m);
 int jl_model_free(jl_model *m);
 /* KvBuffer lifecycle (KvBufferCache.getKvBuffer / close) */
@@ -501,7 +502,10 @@ int jl_model_read_hidden(jl_model *m, int session, float *out /* [embedding_leng
  * which: 0 = x (hidden after the last layer), 1 = xb (after attention + residual), 2 = q, 3 = k, 4 = v (raw projections),
  * 5 = att (attention output), 6 = h (silu(gate) * up; in a mixture-of-experts model [max_batch][experts_per_token][H], expert i of row b
  * at row b * experts_per_token + i), 7 = logits, and for mixture-of-experts models only (JL_ERR_INVALID otherwise) 8 = the router
- * probabilities [max_batch][num_experts] and 9 = the selected experts [max_batch][experts_per_token] as int32 bit patterns. */
+ * probabilities [max_batch][num_experts] and 9 = the selected experts [max_batch][experts_per_token] as int32 bit patterns;
+ * for tensor-core prefill models only 10 = the up projection [max_batch][H] and 11 = the BF16 operand buffer (two BF16 per float
+ * word); for GPT-2 models only 12 = the LayerNorm output [max_batch][E]: ln_2 of the last layer (the c_fc input) after a prompt
+ * forward, ln_f of the sampled rows (the lm_head input) after a decode step or a sampling call. */
 int jl_model_debug_read(jl_model *m, int which, float *out, int64_t n);
 /* diagnostic: CTA 0's phase stamps (globaltimer ns) of the last persistent decode launch (tools/ptrace.py); phase tracing
  * is enabled with JL_PD_TRACE=1 in the environment when the model is created.  Returns the number of words written. */

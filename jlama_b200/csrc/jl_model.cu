@@ -436,7 +436,21 @@ extern "C" int jl_model_finalize(jl_model *m) {
         if (m->n_exp == 0 && c.arch != JL_ARCH_GPT2 && lw[JL_L_UP].dtype != lw[JL_L_GATE].dtype)
             return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "model_finalize: layer %d gate/up weights must share one dtype (got %d/%d)", L,
                                 lw[JL_L_GATE].dtype, lw[JL_L_UP].dtype);
+        // gate/up run fused with SiLU * up, which only the quantised GEMVs implement: refuse F32 / BF16 gate/up here rather than
+        // fail at the first token
+        if (m->n_exp == 0 && c.arch != JL_ARCH_GPT2 && lw[JL_L_GATE].dtype != JL_Q4 && lw[JL_L_GATE].dtype != JL_I8)
+            return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "model_finalize: layer %d slot %d (gate) and slot %d (up): dtype %d, SiLU * up needs Q4 or I8 weights",
+                                L, JL_L_GATE, JL_L_UP, lw[JL_L_GATE].dtype);
     }
+    // the experts' w1 / w3 run fused with SiLU * up the same way, and every expert GEMV decodes one quantised dtype
+    for (int L = 0; L < c.num_layers && m->n_exp > 0; L++)
+        for (int e = c.tp_rank; e < m->n_exp; e += c.tp_size)
+            for (int w = 0; w < 3; w++) {
+                const int dt = m->moe_w[((size_t)L * m->n_exp + e) * 3 + w].dtype;
+                if (dt != JL_Q4 && dt != JL_I8)
+                    return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "model_finalize: layer %d expert %d weight %d (w%d): dtype %d, expert GEMVs need Q4 or I8",
+                                        L, e, w, w + 1, dt);
+            }
     if (c.arch == JL_ARCH_GPT2) {
         for (size_t i = 0; i < m->aux_set.size(); i++)
             if (!m->aux_set[i]) return jl_set_error(ctx, JL_ERR_INVALID, "model_finalize: layer %zu bias slot %zu missing", i / 8, i % 8);
@@ -2659,16 +2673,19 @@ extern "C" int jl_model_debug_read(jl_model *m, int which, float *out, int64_t n
     jl_ctx *ctx = m->ctx;
     JL_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
     // 8 / 9: the router probabilities (the route kernel overwrites the logits) and the selections (int32 bits) of MoE models;
-    // 10 / 11: the up projection and the BF16 operand buffer (uint16 pairs per word) of tensor-core prefill models
-    const float *src[12] = {m->x, m->xb, m->q, m->k, m->v, m->att, m->hbuf, m->logits, m->moe_logits, (const float *)m->moe_sel, m->hbuf2,
-                            (const float *)m->abf};
+    // 10 / 11: the up projection and the BF16 operand buffer (uint16 pairs per word) of tensor-core prefill models;
+    // 12: the LayerNorm output of GPT-2 models (the input of the projection after a LayerNorm: c_fc after a forward, the lm_head
+    // after a sampling call)
+    const float *src[13] = {m->x, m->xb, m->q, m->k, m->v, m->att, m->hbuf, m->logits, m->moe_logits, (const float *)m->moe_sel, m->hbuf2,
+                            (const float *)m->abf, m->cfg.arch == JL_ARCH_GPT2 ? m->ln : nullptr};
     const size_t B = m->maxB;
     size_t kmax = m->cfg.embedding_length > m->h_seg ? m->cfg.embedding_length : m->h_seg;
     if ((size_t)m->attn_seg > kmax) kmax = m->attn_seg;
-    const size_t cap[12] = {B * m->cfg.embedding_length, B * m->cfg.embedding_length, B * m->attn_seg, B * m->kv_seg, B * m->kv_seg,
+    const size_t cap[13] = {B * m->cfg.embedding_length, B * m->cfg.embedding_length, B * m->attn_seg, B * m->kv_seg, B * m->kv_seg,
                             B * m->attn_seg, B * (m->n_exp > 0 ? (size_t)m->exp_k * m->cfg.hidden_length : m->h_seg),
-                            (size_t)m->cfg.max_sessions * m->cfg.vocab_size, B * m->n_exp, B * m->exp_k, B * m->h_seg, B * kmax / 2};
-    if (which < 0 || which > 11 || (size_t)n > cap[which] || !src[which])
+                            (size_t)m->cfg.max_sessions * m->cfg.vocab_size, B * m->n_exp, B * m->exp_k, B * m->h_seg, B * kmax / 2,
+                            B * m->cfg.embedding_length};
+    if (which < 0 || which > 12 || (size_t)n > cap[which] || !src[which])
         return jl_set_error(ctx, JL_ERR_INVALID, "debug_read: bad buffer / size");
     JL_CUDA_CHECK(ctx, cudaStreamSynchronize(m->stream));
     JL_CUDA_CHECK(ctx, cudaMemcpy(out, src[which], (size_t)n * 4, cudaMemcpyDeviceToHost));

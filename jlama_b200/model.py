@@ -529,7 +529,9 @@ class LlamaModel:
         8 is the router probabilities [rows, experts] and 9 the selected experts [rows, experts_per_token] (int32 bits: .view(np.int32)).
         Tensor-core prefill models (prefill_tensor_core=1): 10 is the up projection [rows, H] (h holds the gate projection there),
         and 11 the BF16 operand buffer of the last GEMM, n float words of two BF16 each (.view(np.uint16)); after a tensor-core pass
-        it holds bf16(silu(gate) * up) of the last layer [rows, H], down_proj's input.  Other models refuse 10 and 11."""
+        it holds bf16(silu(gate) * up) of the last layer [rows, H], down_proj's input.  Other models refuse 10 and 11.
+        GPT-2 models: 12 is the LayerNorm output [rows, E]; after batch_forward / batch_forward_multi it holds ln_2 of the last layer
+        (the c_fc input), after decode / sample / sample_multi ln_f of the sampled rows (the lm_head input).  Other models refuse 12."""
         out = np.empty(n, dtype=np.float32)
         self.ctx.check(self.lib.jl_model_debug_read(self.h, which, ptr(out), n))
         return out
