@@ -151,185 +151,84 @@ __global__ void __launch_bounds__(GEMV_THREADS, MINB) gemv_kernel(const GemvPara
 }
 
 // ---- decode kernel: M = 1, Q8 activations, prologue fixed at compile time, one big CTA per SM -----------------------
-// Work split: output rows are dealt to the CTAs; inside a CTA the (row, weight-row, chunk) items are dealt to the warps.
-// LONG = false (a weight row is one chunk, K <= 1024*CH): whole rows go to warps, a warp finishes its rows alone.
-// LONG = true (down_proj: K = 14336 = 3.5 chunks): rows are split at chunk granularity, so every warp streams the same
-// number of bytes (+-1 chunk) however few rows the CTA has; a warp leaves one partial sum per (row, weight-row) it
-// touched in shared memory and, after a barrier, one thread per output row adds the partials in chunk order
-// (deterministic).  The kernel is kept small on purpose: five different kernels alternate every ~50 us, each starts
-// with a cold instruction cache, and every kilobyte on the prologue path showed up in the timeline (tools/ktrace.py).
+// The pass is gemv_phase (jl_gemv_body.cuh).  The kernel is kept small on purpose: five different kernels alternate every
+// ~50 us, each starts with a cold instruction cache, and every kilobyte on the prologue path showed up in the timeline
+// (tools/ktrace.py).
 
-template <int WDT, int EPI, int PRO, int CH, int NBUF, int NT, bool LONG>
-__global__ void __launch_bounds__(NT, 1) gemv_decode_kernel(const GemvParams p, const int) {
-    extern __shared__ __align__(16) unsigned char smem[];
-    constexpr int NWARP = NT / 32;
-    constexpr bool NORM = PRO == PRO_RMSNORM_QUANT;
-    constexpr int NW = (EPI == EPI_SILU_MUL) ? 2 : 1; // weight rows per output row
-    constexpr int WB = (WDT == JL_Q4) ? 16 : 32;      // weight bytes per 32-element block
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int nblk = p.K / 32;
-    const int nchunks = LONG ? (nblk + 32 * CH - 1) / (32 * CH) : 1;
-    ktrace_begin(p.trace, 0x100u | (unsigned)EPI | ((unsigned long long)PRO << 4) | ((unsigned long long)p.total_rows << 16) |
-                              ((unsigned long long)p.K << 40));
-    if (gemv_absent<EPI>(p)) return; // expert held by another rank
-
-    // rows of this CTA, items of this warp
-    const int R0 = (int)(((long long)p.total_rows * blockIdx.x) / gridDim.x);
-    const int R1 = (int)(((long long)p.total_rows * (blockIdx.x + 1)) / gridDim.x);
-    const int nrows = R1 - R0;
-    const int per_row = NW * nchunks;
-    const int items = nrows * per_row;
-    int i0, i1;
-    if (LONG) {
-        i0 = (int)(((long long)items * warp) / NWARP);
-        i1 = (int)(((long long)items * (warp + 1)) / NWARP);
-    } else {
-        i0 = (int)(((long long)nrows * warp) / NWARP) * per_row;
-        i1 = (int)(((long long)nrows * (warp + 1)) / NWARP) * per_row;
+// gemv_phase's view of a launch: segments and MoE pointer tables, the hidden row staged (and normalised) around the ring
+// priming, and the epilogue into the segment's output
+template <int WDT, int EPI, int PRO, int NT, bool LONG>
+struct DecodeGemv {
+    static constexpr bool NORM = PRO == PRO_RMSNORM_QUANT, XLONG = LONG && !NORM;
+    using Stage = StageRegs<NORM, XLONG>;
+    const GemvParams &p;
+    // The hidden row, in flight while the ring is primed.  A separate object: its arrays are indexed in loops that are not
+    // unrolled yet when the compiler first splits up this struct, which would keep `p` in memory until then as well and
+    // move every parameter load of the kernel.
+    Stage &sr;
+    size_t row_blocks, col_blocks; // weight row stride and column offset in 32-element blocks, set by begin()
+    __device__ __forceinline__ DecodeGemv(const GemvParams &p_, Stage &sr_) : p(p_), sr(sr_) {}
+    __device__ __forceinline__ int tid() const { return threadIdx.x; }
+    __device__ __forceinline__ unsigned cta() const { return blockIdx.x; }
+    __device__ __forceinline__ unsigned ncta() const { return gridDim.x; }
+    __device__ __forceinline__ int K() const { return p.K; }
+    __device__ __forceinline__ int rows() const { return p.total_rows; }
+    __device__ __forceinline__ bool begin() {
+        ktrace_begin(p.trace, 0x100u | (unsigned)EPI | ((unsigned long long)PRO << 4) | ((unsigned long long)p.total_rows << 16) |
+                                  ((unsigned long long)p.K << 40));
+        if (gemv_absent<EPI>(p)) return false; // expert held by another rank
+        row_blocks = (size_t)(p.ldw / 32), col_blocks = (size_t)(p.w_col_off / 32);
+        return true;
     }
-    // load cursor: (row relative to R0, weight-row, chunk) plus the byte/element offset of that weight row
-    struct It {
-        int r, wr, c;
-    };
-    const size_t row_blocks = (size_t)(p.ldw / 32), col_blocks = (size_t)(p.w_col_off / 32);
-    auto row_ptrs = [&](const It &it, const uint8_t *&wrow, const float *&srow) {
+    __device__ __forceinline__ void end() const {
+        if (p.trace) {
+            __syncthreads();
+            ktrace_end(p.trace);
+        }
+    }
+    __device__ __forceinline__ void row_ptrs(int row, int wr, int, const uint8_t *&wrow, const float *&srow) const {
         int seg, local;
         if (EPI == EPI_SILU_MUL) {
-            seg = it.wr;
-            local = R0 + it.r;
+            seg = wr;
+            local = row;
         } else {
-            seg_lookup(p, R0 + it.r, seg, local);
+            seg_lookup(p, row, seg, local);
         }
         const size_t blk = (size_t)(p.row0 + local) * row_blocks + col_blocks;
         const void *wb;
         const float *wsb;
         gemv_seg_base(p, seg, wb, wsb);
-        wrow = (const uint8_t *)wb + blk * WB;
+        wrow = (const uint8_t *)wb + blk * (WDT == JL_Q4 ? 16 : 32);
         srow = wsb + blk;
-    };
-    auto advance = [&](It &it) {
-        if (!LONG || ++it.c == nchunks) {
-            it.c = 0;
-            if (++it.wr == NW) {
-                it.wr = 0;
-                ++it.r;
-            }
-        }
-    };
-    It cur, ld;
-    {
-        cur.r = i0 / per_row;
-        const int rem = i0 - cur.r * per_row;
-        cur.wr = rem / nchunks;
-        cur.c = rem - cur.wr * nchunks;
-        ld = cur;
     }
-
-    StageRegs<NORM, LONG && !NORM> sr;
-    WBuf<WDT, CH> buf[NBUF];
-    const uint8_t *wrow;
-    const float *srow;
-    const unsigned long long pol = l2_evict_first_policy();
-    int ci = i0, li = i0;
     // the hidden row (and the norm weights) are requested before this SM's ~80 KB of weight requests
-    stage_q8_issue<NORM, LONG && !NORM, NT>(p, sr);
-#pragma unroll
-    for (int b = 0; b < NBUF - 1; b++) {
-        if (li < i1) {
-            row_ptrs(ld, wrow, srow);
-            load_chunk<WDT, CH>(buf[b], wrow, srow, ld.c * 32 * CH, nblk, lane, pol);
-            advance(ld);
-            li++;
-        }
+    template <class Buf>
+    __device__ __forceinline__ void prime_begin(Buf &) {
+        stage_q8_issue<NORM, XLONG, NT>(p, sr);
     }
-    stage_q8_finish<NORM, LONG && !NORM, NT>(p, sr, smem, nblk);
-    ktrace_mid(p.trace);
+    __device__ __forceinline__ void prime_end(unsigned char *smem, int nblk) {
+        stage_q8_finish<NORM, XLONG, NT>(p, sr, smem, nblk);
+        ktrace_mid(p.trace);
+    }
+    __device__ __forceinline__ void cta_bar() const { __syncthreads(); }
+    __device__ __forceinline__ void store_row(int row, float v0, float v1) const {
+        int seg = 0, local = row;
+        if (EPI != EPI_SILU_MUL) seg_lookup(p, row, seg, local);
+        const GemvSeg &sg = p.seg[seg];
+        float v = EPI == EPI_SILU_MUL ? v1 : v0;
+        if (EPI == EPI_ADD_RESIDUAL) v = __fadd_rn(v, p.residual[p.row0 + local]);
+        if (EPI == EPI_SILU_MUL) v = __fmul_rn(silu_ref(v0), v);
+        sg.out[p.row0 + local + sg.out_off] = v;
+    }
+};
 
-    float *parts = (float *)(smem + (((size_t)nblk * 40 + 15) & ~(size_t)15));
-    const int maxsplit = nchunks < NWARP ? nchunks : NWARP;
-    float acc[1] = {0.0f};
-    // !LONG: finished rows are parked one per lane (lane i holds the i-th finished row of this warp) and the epilogue --
-    // residual add or the double-precision SiLU -- runs for all parked rows at once with coalesced stores, instead of
-    // lane 0 doing it serially after every row (gate+up: 18.7 vs 19.9 us per launch)
-    float park0 = 0.0f, park1 = 0.0f; // value (or gate), up
-    int nparked = 0, park_row0 = R0 + cur.r;
-    auto flush = [&]() {
-        if (lane < nparked) {
-            int seg = 0, local = park_row0 + lane;
-            if (EPI != EPI_SILU_MUL) seg_lookup(p, park_row0 + lane, seg, local);
-            const GemvSeg &sg = p.seg[seg];
-            float v = NW == 2 ? park1 : park0;
-            if (EPI == EPI_ADD_RESIDUAL) v = __fadd_rn(v, p.residual[p.row0 + local]);
-            if (EPI == EPI_SILU_MUL) v = __fmul_rn(silu_ref(park0), v);
-            sg.out[p.row0 + local + sg.out_off] = v;
-        }
-        park_row0 += nparked;
-        nparked = 0;
-    };
-    while (ci < i1) {
-#pragma unroll
-        for (int b = 0; b < NBUF; b++) {
-            if (ci < i1) {
-                if (li < i1) {
-                    row_ptrs(ld, wrow, srow);
-                    load_chunk<WDT, CH>(buf[(b + NBUF - 1) % NBUF], wrow, srow, ld.c * 32 * CH, nblk, lane, pol);
-                    advance(ld);
-                    li++;
-                }
-                compute_chunk<WDT, true, 1, CH>(buf[b], acc, smem, cur.c * 32 * CH, nblk, lane);
-                if (!LONG) {
-                    const float v = warp_sum(acc[0]); // every lane has the total
-                    acc[0] = 0.0f;
-                    if (NW == 2 && cur.wr == 0) {
-                        if (lane == nparked) park0 = v;
-                    } else {
-                        if (lane == nparked) (NW == 2 ? park1 : park0) = v;
-                        ++nparked;
-                    }
-                } else if (cur.c == nchunks - 1 || ci == i1 - 1) {
-                    // partial of (row, weight-row) from this warp
-                    const float v = warp_sum(acc[0]);
-                    const int rw = cur.r * NW + cur.wr;
-                    // slot: with at least one item per warp the row's owners are consecutive warps; with fewer items than warps
-                    // (a launch of few rows) each warp owns at most one item, so its chunk is its slot (owners are not consecutive)
-                    const int slot = items >= NWARP ? warp - item_owner(rw * nchunks, items, NWARP) : cur.c;
-                    if (lane == 0) parts[rw * maxsplit + slot] = v;
-                    acc[0] = 0.0f;
-                }
-                advance(cur);
-                ci++;
-            }
-        }
-        if (!LONG && nparked > 32 - NBUF) flush(); // checked once per ring revolution: at most NBUF rows arrive in between
-    }
-    if (!LONG) flush();
-    if (LONG) {
-        __syncthreads();
-        for (int o = tid; o < nrows; o += NT) {
-            float sums[NW];
-#pragma unroll
-            for (int wr = 0; wr < NW; wr++) {
-                const int rw = o * NW + wr;
-                const int wa = items >= NWARP ? item_owner(rw * nchunks, items, NWARP) : 0;
-                const int ns = items >= NWARP ? item_owner(rw * nchunks + nchunks - 1, items, NWARP) - wa + 1 : nchunks;
-                float t = 0.0f;
-                for (int s = 0; s < ns; s++) t = __fadd_rn(t, parts[rw * maxsplit + s]);
-                sums[wr] = t;
-            }
-            int seg = 0, local = R0 + o;
-            if (EPI != EPI_SILU_MUL) seg_lookup(p, R0 + o, seg, local);
-            const GemvSeg &sg = p.seg[seg];
-            const int col = p.row0 + local + sg.out_off;
-            float v = sums[NW - 1];
-            if (EPI == EPI_ADD_RESIDUAL) v = __fadd_rn(v, p.residual[p.row0 + local]);
-            if (EPI == EPI_SILU_MUL) v = __fmul_rn(silu_ref(sums[0]), v);
-            sg.out[col] = v;
-        }
-    }
-    if (p.trace) {
-        __syncthreads();
-        ktrace_end(p.trace);
-    }
+template <int WDT, int EPI, int PRO, int CH, int NBUF, int NT, bool LONG>
+__global__ void __launch_bounds__(NT, 1) gemv_decode_kernel(const GemvParams p, const int) {
+    extern __shared__ __align__(16) unsigned char smem[];
+    using Ph = DecodeGemv<WDT, EPI, PRO, NT, LONG>;
+    typename Ph::Stage sr;
+    Ph ph(p, sr);
+    gemv_phase<Ph, WDT, EPI, CH, NBUF, NT, LONG>(ph, smem);
 }
 
 // ---- dense (F32 / BF16 weights) GEMV: GemmerF32 / GemmerF32BF16 (PanamaTensorOperations.java:1046-1231,1466-1539)
@@ -452,7 +351,7 @@ static int launch_decode_k(jl_ctx *ctx, cudaStream_t stream, const GemvParams &p
 }
 
 template <int WDT, int EPI, int PRO, int NT, int NBUF, int CH>
-static int launch_decode(jl_ctx *ctx, cudaStream_t stream, const GemvParams &p, size_t smem) {
+static int launch_decode(jl_ctx *ctx, cudaStream_t stream, const GemvParams &p) {
     if (PRO == PRO_RMSNORM_QUANT && p.K > 16 * NT)
         return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "gemv: RMSNorm prologue supports rows up to %d", 16 * NT);
     int grid = ctx->sm_count;
@@ -460,8 +359,8 @@ static int launch_decode(jl_ctx *ctx, cudaStream_t stream, const GemvParams &p, 
     if (grid > max_grid) grid = max_grid;
     const int nchunks = (p.K / 32 + 32 * CH - 1) / (32 * CH);
     const bool lng = nchunks > 1;
-    size_t smem_d = ((smem + 15) & ~(size_t)15);
-    if (lng) { // partial sums of split rows live behind the staged activations
+    size_t smem_d = gemv_parts_offset(p.K / 32);
+    if (lng) {
         const int rows_per_cta = (p.total_rows + grid - 1) / grid;
         const int maxsplit = nchunks < NT / 32 ? nchunks : NT / 32;
         smem_d += (size_t)rows_per_cta * (EPI == EPI_SILU_MUL ? 2 : 1) * maxsplit * 4;
@@ -479,9 +378,9 @@ static int launch_q(jl_ctx *ctx, cudaStream_t stream, const GemvParams &p, int p
         //   704 x 2: 5.98 / 4.62 / 15.93 / 11.10    768 x 2: 6.17 / 4.77 / 16.07 / 11.12    384 x 4: 6.32 / 4.75 / 17.01 / 11.42
         // The long gate+up stream wants warps (issue slots), the short launches want the deeper ring.
         constexpr int NT = EPI == EPI_SILU_MUL ? 640 : 512, NB = EPI == EPI_SILU_MUL ? 2 : 3;
-        if (prologue == PRO_F32_QUANT) return launch_decode<WDT, EPI, PRO_F32_QUANT, NT, NB, 4>(ctx, stream, p, smem);
+        if (prologue == PRO_F32_QUANT) return launch_decode<WDT, EPI, PRO_F32_QUANT, NT, NB, 4>(ctx, stream, p);
         if (prologue == PRO_RMSNORM_QUANT && p.K <= 16 * NT)
-            return launch_decode<WDT, EPI, PRO_RMSNORM_QUANT, NT, NB, 4>(ctx, stream, p, smem);
+            return launch_decode<WDT, EPI, PRO_RMSNORM_QUANT, NT, NB, 4>(ctx, stream, p);
     }
     constexpr int MINB = (MM <= 2) ? 2 : 1;
     static size_t cfg[JL_MAX_DEVICES] = {};

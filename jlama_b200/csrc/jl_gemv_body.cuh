@@ -1,5 +1,6 @@
 // Device code shared by the quantised GEMV kernels (jl_gemv.cu) and the persistent decode kernel (jl_pdecode.cu):
-// register chunk buffers, weight loads, activation staging (RMSNorm / Q8 quantiser) and the per-chunk dot products.
+// register chunk buffers, weight loads, activation staging (RMSNorm / Q8 quantiser), the per-chunk dot products and the
+// M = 1 decode pass built from them (gemv_phase).
 // Everything here is header-only device code; see jl_gemv.cu for the design notes and the reference citations.
 #pragma once
 #include "jl_common.cuh"
@@ -68,7 +69,8 @@ __device__ __forceinline__ void load_chunk(WBuf<WDT, CH> &b, const uint8_t *wrow
 // ---- activation staging -------------------------------------------------------------------------
 // Q8 layout in smem:  q[m][half][blk][16] int8, then sc[m][blk] f32, then sum[m][blk] int32
 // F32 layout in smem: f[m][c4(8)][blk][4] floats
-__device__ __forceinline__ size_t q8_bytes_per_row(int nblk) { return (size_t)nblk * 32 + (size_t)nblk * 8; }
+// gemv_phase (M = 1) keeps the partial sums of its LONG rows behind the Q8 row, from this 16-byte aligned offset
+__host__ __device__ __forceinline__ size_t gemv_parts_offset(int nblk) { return ((size_t)nblk * 40 + 15) & ~(size_t)15; }
 
 // One thread owns one 32-element block: 8 independent 128-bit loads, the block max, the Q8 rounding
 // and the packing all stay in registers (no shuffles), so the prologue costs about one L2 round trip.
@@ -512,5 +514,157 @@ __device__ __forceinline__ void compute_chunk(const WBuf<WDT, CH> &w, float (&ac
             }
         }
     }
+}
+
+// ---- one M = 1 GEMV pass over quantised weights with Q8 activations -----------------------------------------------
+// The body of gemv_decode_kernel (jl_gemv.cu) and of every GEMV phase of the persistent decode kernel (jl_pdecode.cu).
+// Work split: output rows are dealt to the CTAs; inside a CTA the (row, weight-row, chunk) items are dealt to the warps.
+// LONG = false (a weight row is one chunk, K <= 1024*CH): whole rows go to warps, a warp finishes its rows alone.
+// LONG = true (down_proj: K = 14336 = 3.5 chunks): rows are split at chunk granularity, so every warp streams the same
+// number of bytes (+-1 chunk) however few rows the CTA has; a warp leaves one partial sum per (row, weight-row) it
+// touched in shared memory and, after a barrier, one thread per output row adds the partials in chunk order
+// (deterministic).
+//
+// Ph supplies, as inline methods, what differs between the two kernels:
+//   tid(), cta(), ncta()                     thread id, CTA id and grid size (the persistent kernel's are opaque copies)
+//   K(), rows()                              reduction length and output rows of the pass
+//   begin(), end()                           first and last code of the pass; begin() == false skips the pass and end()
+//   row_ptrs(row, wr, nblk, wrow, srow)      weight and scale row of weight-row wr (gate / up) of output row `row`
+//   prime_begin(buf), prime_end(smem, nblk)  before and after the ring is primed: activation staging, dependency waits
+//   cta_bar()                                the CTA barrier before the LONG partials are combined
+//   store_row(row, v0, v1)                   epilogue of one output row (v0 = value or gate, v1 = up)
+// Each hook runs where the kernel ran that code before the two passes were merged: moving any of it changes the
+// compiled kernels.
+template <class Ph, int WDT, int EPI, int CH, int NBUF, int NT, bool LONG>
+__device__ __forceinline__ void gemv_phase(Ph &ph, unsigned char *smem) {
+    constexpr int NWARP = NT / 32;
+    constexpr int NW = (EPI == EPI_SILU_MUL) ? 2 : 1; // weight rows per output row
+    const int tid = ph.tid(), lane = tid & 31, warp = tid >> 5;
+    const int nblk = ph.K() / 32;
+    const int nchunks = LONG ? (nblk + 32 * CH - 1) / (32 * CH) : 1;
+    if (!ph.begin()) return;
+
+    // rows of this CTA, items of this warp
+    const int R0 = (int)(((long long)ph.rows() * ph.cta()) / ph.ncta());
+    const int R1 = (int)(((long long)ph.rows() * (ph.cta() + 1)) / ph.ncta());
+    const int nrows = R1 - R0;
+    const int per_row = NW * nchunks;
+    const int items = nrows * per_row;
+    int i0, i1;
+    if (LONG) {
+        i0 = (int)(((long long)items * warp) / NWARP);
+        i1 = (int)(((long long)items * (warp + 1)) / NWARP);
+    } else {
+        i0 = (int)(((long long)nrows * warp) / NWARP) * per_row;
+        i1 = (int)(((long long)nrows * (warp + 1)) / NWARP) * per_row;
+    }
+    // cursor: (row relative to R0, weight-row, chunk)
+    struct It {
+        int r, wr, c;
+    };
+    auto row_ptrs = [&](const It &it, const uint8_t *&wrow, const float *&srow) { ph.row_ptrs(R0 + it.r, it.wr, nblk, wrow, srow); };
+    auto advance = [&](It &it) {
+        if (!LONG || ++it.c == nchunks) {
+            it.c = 0;
+            if (++it.wr == NW) {
+                it.wr = 0;
+                ++it.r;
+            }
+        }
+    };
+    It cur, ld;
+    {
+        cur.r = i0 / per_row;
+        const int rem = i0 - cur.r * per_row;
+        cur.wr = rem / nchunks;
+        cur.c = rem - cur.wr * nchunks;
+        ld = cur;
+    }
+
+    WBuf<WDT, CH> buf[NBUF];
+    // NBUF-1 chunks per warp go in flight before the activations are staged: the weight stream does not depend on them
+    ph.prime_begin(buf);
+    const uint8_t *wrow;
+    const float *srow;
+    const unsigned long long pol = l2_evict_first_policy();
+    int ci = i0, li = i0;
+#pragma unroll
+    for (int b = 0; b < NBUF - 1; b++) {
+        if (li < i1) {
+            row_ptrs(ld, wrow, srow);
+            load_chunk<WDT, CH>(buf[b], wrow, srow, ld.c * 32 * CH, nblk, lane, pol);
+            advance(ld);
+            li++;
+        }
+    }
+    ph.prime_end(smem, nblk);
+
+    float *parts = (float *)(smem + gemv_parts_offset(nblk));
+    const int maxsplit = nchunks < NWARP ? nchunks : NWARP;
+    float acc[1] = {0.0f};
+    // !LONG: finished rows are parked one per lane (lane i holds the i-th finished row of this warp) and the epilogue --
+    // residual add or the double-precision SiLU -- runs for all parked rows at once with coalesced stores, instead of
+    // lane 0 doing it serially after every row (gate+up: 18.7 vs 19.9 us per launch)
+    float park0 = 0.0f, park1 = 0.0f; // value (or gate), up
+    int nparked = 0, park_row0 = R0 + cur.r;
+    auto flush = [&]() {
+        if (lane < nparked) ph.store_row(park_row0 + lane, park0, park1);
+        park_row0 += nparked;
+        nparked = 0;
+    };
+    while (ci < i1) {
+#pragma unroll
+        for (int b = 0; b < NBUF; b++) {
+            if (ci < i1) {
+                if (li < i1) {
+                    row_ptrs(ld, wrow, srow);
+                    load_chunk<WDT, CH>(buf[(b + NBUF - 1) % NBUF], wrow, srow, ld.c * 32 * CH, nblk, lane, pol);
+                    advance(ld);
+                    li++;
+                }
+                compute_chunk<WDT, true, 1, CH>(buf[b], acc, smem, cur.c * 32 * CH, nblk, lane);
+                if (!LONG) {
+                    const float v = warp_sum(acc[0]); // every lane has the total
+                    acc[0] = 0.0f;
+                    if (NW == 2 && cur.wr == 0) {
+                        if (lane == nparked) park0 = v;
+                    } else {
+                        if (lane == nparked) (NW == 2 ? park1 : park0) = v;
+                        ++nparked;
+                    }
+                } else if (cur.c == nchunks - 1 || ci == i1 - 1) {
+                    // partial of (row, weight-row) from this warp
+                    const float v = warp_sum(acc[0]);
+                    const int rw = cur.r * NW + cur.wr;
+                    // slot: with at least one item per warp the row's owners are consecutive warps; with fewer items than warps
+                    // (a launch of few rows) each warp owns at most one item, so its chunk is its slot (owners are not consecutive)
+                    const int slot = items >= NWARP ? warp - item_owner(rw * nchunks, items, NWARP) : cur.c;
+                    if (lane == 0) parts[rw * maxsplit + slot] = v;
+                    acc[0] = 0.0f;
+                }
+                advance(cur);
+                ci++;
+            }
+        }
+        if (!LONG && nparked > 32 - NBUF) flush(); // checked once per ring revolution: at most NBUF rows arrive in between
+    }
+    if (!LONG) flush();
+    if (LONG) {
+        ph.cta_bar();
+        for (int o = tid; o < nrows; o += NT) {
+            float sums[NW];
+#pragma unroll
+            for (int wr = 0; wr < NW; wr++) {
+                const int rw = o * NW + wr;
+                const int wa = items >= NWARP ? item_owner(rw * nchunks, items, NWARP) : 0;
+                const int ns = items >= NWARP ? item_owner(rw * nchunks + nchunks - 1, items, NWARP) - wa + 1 : nchunks;
+                float t = 0.0f;
+                for (int s = 0; s < ns; s++) t = __fadd_rn(t, parts[rw * maxsplit + s]);
+                sums[wr] = t;
+            }
+            ph.store_row(R0 + o, sums[0], sums[NW - 1]);
+        }
+    }
+    ph.end();
 }
 

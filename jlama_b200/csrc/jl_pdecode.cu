@@ -41,9 +41,6 @@
 #define PD_SPIN_LOCAL (1u << 22)
 #define PD_SPIN_PEER (1u << 26)
 #define EPI_LL 3 // partial sums to every rank's LL receive buffer (tensor parallel o_proj / down_proj)
-#ifndef PD_PHASE_FN
-#define PD_PHASE_FN __forceinline__
-#endif
 
 // ---- model constants ----------------------------------------------------------------------------------------------------
 // Everything a phase needs -- dims, buffers, per-layer weight pointers -- lives in __constant__ memory, so the phase bodies use
@@ -181,178 +178,87 @@ __device__ __forceinline__ void pd_ring_clear(WBuf<WDT, CH> (&buf)[NBUF]) {
 }
 
 // ---- one quantised GEMV phase (M = 1, Q8 activations) -------------------------------------------------------------------
-// Work split as in gemv_decode_kernel (jl_gemv.cu): output rows are dealt to the CTAs, inside a CTA the (row, weight-row,
-// chunk) items to the warps; LONG rows (longer than one register chunk) are split at chunk granularity with per-warp partial
-// sums combined in chunk order.  The ring is primed BEFORE the dependency counter is polled.
-// __noinline__: every phase gets its own register allocation (inlined into one kernel the ring buffers spilled).
+// The pass is gemv_phase (jl_gemv_body.cuh).  The ring is primed BEFORE the dependency counter is polled.
+// gemv_phase's view of a phase: the layer's weights and activations from constant memory, the dependency wait between ring
+// priming and staging, and the epilogue into the phase's output or (EPI_LL) every rank's receive buffer
 template <int WDT, int PH, int EPI, bool LONG>
-__device__ PD_PHASE_FN void pd_gemv(const int, const int L, const uint32_t tag, const int dep_which, const unsigned long long dep_target,
-                                     const int stamp_idx, unsigned char *smem) {
-    PD_OPAQUE_ZERO(pz);
-    constexpr int NT = PD_NT, NWARP = PD_NWARP, CH = PD_CH(WDT), NBUF = PD_NBUF;
-    constexpr bool NORM = PH == PH_QKV || PH == PH_GU;
-    constexpr int NW = (EPI == EPI_SILU_MUL) ? 2 : 1; // weight rows per output row
-    constexpr int WB = (WDT == JL_Q4) ? 16 : 32;      // weight bytes per 32-element block
-    // The phases are inlined into one loop over the layers and all their index arithmetic (row ranges, item ranges, ...) is
-    // loop-invariant: hoisted out of the layer loop it stayed live across every phase (~60 registers) and the weight ring
-    // spilled to local memory.  An opaque copy of the thread / CTA ids keeps each phase's bookkeeping inside the phase.
-    int tid = threadIdx.x, cta_id = blockIdx.x, ncta = gridDim.x;
-    asm volatile("" : "+r"(tid), "+r"(cta_id), "+r"(ncta));
-    const int lane = tid & 31, warp = tid >> 5;
-    const int nblk = ph_K<PH>(pz) / 32;
-    const int nchunks = LONG ? (nblk + 32 * CH - 1) / (32 * CH) : 1;
-    const int R0 = (int)(((long long)ph_rows<PH>(pz) * cta_id) / ncta);
-    const int R1 = (int)(((long long)ph_rows<PH>(pz) * (cta_id + 1)) / ncta);
-    const int nrows = R1 - R0;
-    const int per_row = NW * nchunks;
-    const int items = nrows * per_row;
-    int i0, i1;
-    if (LONG) {
-        i0 = (int)(((long long)items * warp) / NWARP);
-        i1 = (int)(((long long)items * (warp + 1)) / NWARP);
-    } else {
-        i0 = (int)(((long long)nrows * warp) / NWARP) * per_row;
-        i1 = (int)(((long long)nrows * (warp + 1)) / NWARP) * per_row;
-    }
-    struct It {
-        int r, wr, c;
-    };
-    auto row_ptrs = [&](const It &it, const uint8_t *&wrow, const float *&srow) {
+struct PdGemv {
+    static constexpr bool NORM = PH == PH_QKV || PH == PH_GU, XLONG = LONG && !NORM;
+    int tid_, cta_, ncta_; // opaque copies, see pd_gemv
+    int L;
+    uint32_t tag;
+    int dep_which;
+    unsigned long long dep_target;
+    int stamp_idx;
+    __device__ __forceinline__ int K() const { return ph_K<PH>(0); }
+    __device__ __forceinline__ int rows() const { return ph_rows<PH>(0); }
+    __device__ __forceinline__ int tid() const { return tid_; }
+    __device__ __forceinline__ int cta() const { return cta_; }
+    __device__ __forceinline__ int ncta() const { return ncta_; }
+    __device__ __forceinline__ bool begin() const { return true; }
+    __device__ __forceinline__ void end() const {}
+    __device__ __forceinline__ void row_ptrs(int row, int wr, int nblk, const uint8_t *&wrow, const float *&srow) const {
         int seg, local;
         if (EPI == EPI_SILU_MUL) {
-            seg = it.wr;
-            local = R0 + it.r;
+            seg = wr;
+            local = row;
         } else {
-            ph_seg<PH>(pz, R0 + it.r, seg, local);
+            ph_seg<PH>(0, row, seg, local);
         }
         const uint8_t *w;
         const float *s;
         ph_weights<PH>(L, seg, w, s);
         const size_t blk = (size_t)local * (size_t)nblk;
-        wrow = w + blk * WB;
+        wrow = w + blk * (WDT == JL_Q4 ? 16 : 32);
         srow = s + blk;
-    };
-    auto advance = [&](It &it) {
-        if (!LONG || ++it.c == nchunks) {
-            it.c = 0;
-            if (++it.wr == NW) {
-                it.wr = 0;
-                ++it.r;
-            }
-        }
-    };
-    It cur, ld;
-    {
-        cur.r = i0 / per_row;
-        const int rem = i0 - cur.r * per_row;
-        cur.wr = rem / nchunks;
-        cur.c = rem - cur.wr * nchunks;
-        ld = cur;
     }
-    WBuf<WDT, CH> buf[NBUF];
-    pd_ring_clear<WDT, CH, NBUF>(buf);
-    const uint8_t *wrow;
-    const float *srow;
-    const unsigned long long pol = l2_evict_first_policy();
-    int ci = i0, li = i0;
-#pragma unroll
-    for (int b = 0; b < NBUF - 1; b++) {
-        if (li < i1) {
-            row_ptrs(ld, wrow, srow);
-            load_chunk<WDT, CH>(buf[b], wrow, srow, ld.c * 32 * CH, nblk, lane, pol);
-            advance(ld);
-            li++;
-        }
+    template <int CH, int NBUF>
+    __device__ __forceinline__ void prime_begin(WBuf<WDT, CH> (&buf)[NBUF]) {
+        pd_ring_clear<WDT, CH, NBUF>(buf);
     }
-    pd_wait(pz, dep_which, dep_target);
-    pd_stamp(pz, stamp_idx);
-    {
+    __device__ __forceinline__ void prime_end(unsigned char *smem, int nblk) {
+        PD_OPAQUE_ZERO(pz);
+        pd_wait(pz, dep_which, dep_target);
+        pd_stamp(pz, stamp_idx);
         GemvParams p; // only the staging fields; dead after the prologue
         p.a = PH == PH_QKV ? CP.x : (PH == PH_O ? CP.att : (PH == PH_GU ? CP.xb : CP.h));
         p.a_col_off = 0, p.K = ph_K<PH>(pz), p.lda = p.K;
         p.norm_w = PH == PH_QKV ? c_pd.layers[L].attn_norm : c_pd.layers[L].ffn_norm;
         p.norm_w_dtype = PH == PH_QKV ? c_pd.layers[L].attn_norm_dt : c_pd.layers[L].ffn_norm_dt;
         p.norm_adj = 0.0f, p.norm_eps = CP.eps, p.norm_E = CP.E, p.norm_inv_E = 1.0 / (double)CP.E;
-        StageRegs<NORM, LONG && !NORM> sr;
-        stage_q8_issue<NORM, LONG && !NORM, NT>(p, sr);
-        stage_q8_finish<NORM, LONG && !NORM, NT, 1>(p, sr, smem, nblk);
+        StageRegs<NORM, XLONG> sr;
+        stage_q8_issue<NORM, XLONG, PD_NT>(p, sr);
+        stage_q8_finish<NORM, XLONG, PD_NT, 1>(p, sr, smem, nblk);
     }
-    float *parts = (float *)(smem + (((size_t)nblk * 40 + 15) & ~(size_t)15));
-    const int maxsplit = nchunks < NWARP ? nchunks : NWARP;
-    float acc[1] = {0.0f};
-    float park0 = 0.0f, park1 = 0.0f; // value (or gate), up
-    int nparked = 0, park_row0 = R0 + cur.r;
-    auto store_row = [&](int row, float v0, float v1) { // row = index in the concatenated row space of the phase
+    __device__ __forceinline__ void cta_bar() const { pd_cta_bar(); }
+    // row = index in the concatenated row space of the phase
+    __device__ __forceinline__ void store_row(int row, float v0, float v1) const {
+        PD_OPAQUE_ZERO(pz);
         int seg = 0, local = row;
         if (EPI != EPI_SILU_MUL) ph_seg<PH>(pz, row, seg, local);
-        float v = NW == 2 ? v1 : v0;
+        float v = EPI == EPI_SILU_MUL ? v1 : v0;
         if (EPI == EPI_ADD_RESIDUAL) v = __fadd_rn(v, __ldcg((PH == PH_O ? CP.x : CP.xb) + local));
         if (EPI == EPI_SILU_MUL) v = __fmul_rn(silu_ref(v0), v);
         if (EPI == EPI_LL) ll_store<PH>(pz, local, v, tag);
         else ph_out<PH>(pz, seg)[local] = v;
-    };
-    auto flush = [&]() {
-        if (lane < nparked) store_row(park_row0 + lane, park0, park1);
-        park_row0 += nparked;
-        nparked = 0;
-    };
-    while (ci < i1) {
-#pragma unroll
-        for (int b = 0; b < NBUF; b++) {
-            if (ci < i1) {
-                if (li < i1) {
-                    row_ptrs(ld, wrow, srow);
-                    load_chunk<WDT, CH>(buf[(b + NBUF - 1) % NBUF], wrow, srow, ld.c * 32 * CH, nblk, lane, pol);
-                    advance(ld);
-                    li++;
-                }
-                compute_chunk<WDT, true, 1, CH>(buf[b], acc, smem, cur.c * 32 * CH, nblk, lane);
-                if (!LONG) {
-                    const float v = warp_sum(acc[0]);
-                    acc[0] = 0.0f;
-                    if (NW == 2 && cur.wr == 0) {
-                        if (lane == nparked) park0 = v;
-                    } else {
-                        if (lane == nparked) (NW == 2 ? park1 : park0) = v;
-                        ++nparked;
-                    }
-                } else if (cur.c == nchunks - 1 || ci == i1 - 1) {
-                    const float v = warp_sum(acc[0]);
-                    const int rw = cur.r * NW + cur.wr;
-                    // slot as in gemv_decode_kernel: the owner's offset when every warp owns an item, else the chunk (one item per warp)
-                    const int slot = items >= NWARP ? warp - item_owner(rw * nchunks, items, NWARP) : cur.c;
-                    if (lane == 0) parts[rw * maxsplit + slot] = v;
-                    acc[0] = 0.0f;
-                }
-                advance(cur);
-                ci++;
-            }
-        }
-        if (!LONG && nparked > 32 - NBUF) flush();
     }
-    if (!LONG) flush();
-    if (LONG) {
-        pd_cta_bar();
-        for (int o = tid; o < nrows; o += NT) {
-            float sums[NW];
-#pragma unroll
-            for (int wr = 0; wr < NW; wr++) {
-                const int rw = o * NW + wr;
-                const int wa = items >= NWARP ? item_owner(rw * nchunks, items, NWARP) : 0;
-                const int ns = items >= NWARP ? item_owner(rw * nchunks + nchunks - 1, items, NWARP) - wa + 1 : nchunks;
-                float t = 0.0f;
-                for (int s = 0; s < ns; s++) t = __fadd_rn(t, parts[rw * maxsplit + s]);
-                sums[wr] = t;
-            }
-            store_row(R0 + o, sums[0], sums[NW - 1]);
-        }
-    }
-}
+};
 
+template <int WDT, int PH, int EPI, bool LONG>
+__device__ __forceinline__ void pd_gemv(const int, const int L, const uint32_t tag, const int dep_which, const unsigned long long dep_target,
+                                        const int stamp_idx, unsigned char *smem) {
+    // The phases are inlined into one loop over the layers and all their index arithmetic (row ranges, item ranges, ...) is
+    // loop-invariant: hoisted out of the layer loop it stayed live across every phase (~60 registers) and the weight ring
+    // spilled to local memory.  An opaque copy of the thread / CTA ids keeps each phase's bookkeeping inside the phase.
+    int tid = threadIdx.x, cta_id = blockIdx.x, ncta = gridDim.x;
+    asm volatile("" : "+r"(tid), "+r"(cta_id), "+r"(ncta));
+    PdGemv<WDT, PH, EPI, LONG> ph{tid, cta_id, ncta, L, tag, dep_which, dep_target, stamp_idx};
+    gemv_phase<decltype(ph), WDT, EPI, PD_CH(WDT), PD_NBUF, PD_NT, LONG>(ph, smem);
+}
 
 // ---- lm_head: F32 activations (RMSNorm, not re-quantised: AbstractModel.java:444-449) x quantised rows + running arg-max --
 template <int WDT>
-__device__ PD_PHASE_FN unsigned long long pd_lm_head(const int, const int dep_which, const unsigned long long dep_target, const int stamp_idx,
+__device__ __forceinline__ unsigned long long pd_lm_head(const int, const int dep_which, const unsigned long long dep_target, const int stamp_idx,
                                                      const int want_logits, unsigned char *smem) {
     PD_OPAQUE_ZERO(pz);
     constexpr int NT = PD_NT, NWARP = PD_NWARP, CH = PD_CH(WDT), NBUF = PD_NBUF;
@@ -466,7 +372,7 @@ __device__ __forceinline__ float pd_embed_value(const int pz, size_t tok, int c)
 
 // reduce the LL partials of this CTA's rows in rank order, add the residual, store the new hidden rows (local global)
 template <int PH>
-__device__ PD_PHASE_FN void pd_ll_reduce(const int, uint32_t tag, float *scratch /* smem [rows][world] */) {
+__device__ __forceinline__ void pd_ll_reduce(const int, uint32_t tag, float *scratch /* smem [rows][world] */) {
     PD_OPAQUE_ZERO(pz);
     const int tid = threadIdx.x;
     const int E = CP.E, W = CP.world;
@@ -489,7 +395,7 @@ __device__ PD_PHASE_FN void pd_ll_reduce(const int, uint32_t tag, float *scratch
 
 // One attention task.  qkv_target != 0: the QKV barrier is waited for inside (after the first K/V rows have been requested).
 template <int HS>
-__device__ PD_PHASE_FN void pd_attention(const int, const int layer, const int kvh, const int split, const int splits, const bool merge,
+__device__ __forceinline__ void pd_attention(const int, const int layer, const int kvh, const int split, const int splits, const bool merge,
                                          const unsigned long long qkv_target, unsigned char *smem) {
     PD_OPAQUE_ZERO(pz);
     AttnParams at;
@@ -696,7 +602,7 @@ static size_t pd_smem_bytes(const PdParams &p, int G) {
     if (p.attn_seg > Kmax) Kmax = p.attn_seg;
     int Rmax = p.E > p.H ? p.E : p.H; // rows of the largest phase that may run in the split-row (LONG) form; gate+up has two weight rows
     if (p.attn_seg + 2 * p.kv_seg > Rmax) Rmax = p.attn_seg + 2 * p.kv_seg;
-    size_t acts = (((size_t)(Kmax / 32) * 40 + 15) & ~(size_t)15) + (size_t)((Rmax + G - 1) / G + 2) * 2 * PD_NWARP * 4 + 64;
+    size_t acts = gemv_parts_offset(Kmax / 32) + (size_t)((Rmax + G - 1) / G + 2) * 2 * PD_NWARP * 4 + 64;
     const size_t lm = (size_t)p.E * 4;
     if (lm > acts) acts = lm;
     const int hs = p.head_size;
@@ -755,15 +661,11 @@ static int launch_pd(jl_ctx *ctx, cudaStream_t stream, const PdParams &p) {
 
 template <int WDT>
 static int launch_pd_hs(jl_ctx *ctx, cudaStream_t stream, const PdParams &p) {
-#ifdef PD_EXPERIMENT_ONLY_128
-    return launch_pd<WDT, 128>(ctx, stream, p);
-#else
     switch (p.head_size) {
         case 32: return launch_pd<WDT, 32>(ctx, stream, p);
         case 64: return launch_pd<WDT, 64>(ctx, stream, p);
         default: return launch_pd<WDT, 128>(ctx, stream, p);
     }
-#endif
 }
 
 // `owner`: identity of the model the constants belong to; `layers_host`: its PdLayer table (host copy).
@@ -782,9 +684,5 @@ int jl_launch_pdecode(jl_ctx *ctx, cudaStream_t stream, const PdParams &p, const
             g_pd_owner[d] = owner;
         }
     }
-#ifdef PD_EXPERIMENT_ONLY_128
-    return launch_pd_hs<JL_Q4>(ctx, stream, p);
-#else
     return w_dtype == JL_Q4 ? launch_pd_hs<JL_Q4>(ctx, stream, p) : launch_pd_hs<JL_I8>(ctx, stream, p);
-#endif
 }
