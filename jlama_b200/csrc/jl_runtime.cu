@@ -212,21 +212,27 @@ static int gemm_locked(jl_ctx *ctx, int a_dtype, const void *a, const float *a_s
         return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "gemm: activation dtype %d", a_dtype);
     if (bq && ((k % 32) || (b_col_off % 32) || (a_dtype == JL_I8 && (a_col_off % 32))))
         return jl_set_error(ctx, JL_ERR_INVALID, "gemm: quantised operands need 32-aligned offsets/length");
+    // an I8 row's scales are its lda / 32 block scales: a row stride that is not whole blocks has no scale layout
+    if (a_dtype == JL_I8 && (lda % 32)) return jl_set_error(ctx, JL_ERR_INVALID, "gemm: I8 activations need lda %% 32 == 0 (lda=%d)", lda);
     // the output row slice written by this call: columns [n0-roffset, n0-roffset+n)
     const int c0 = n0 - roffset;
     if (c0 < 0 || c0 + n > ldc) return jl_set_error(ctx, JL_ERR_INVALID, "gemm: result offset out of range");
 
+    // Only the k columns each row uses are uploaded, packed at a row stride of k rounded up to 32 elements: the kernels load
+    // activations 16 bytes at a time, so every row must start 16-byte aligned whatever the caller's column offset and row stride.
     const size_t esz = a_dtype == JL_F32 ? 4 : (a_dtype == JL_BF16 ? 2 : 1);
-    const size_t a_bytes = (size_t)m * lda * esz;
-    void *da = jl_scratch(ctx, 0, a_bytes);
+    const int kp = (k + 31) & ~31;
+    void *da = jl_scratch(ctx, 0, (size_t)m * kp * esz);
     float *dr = (float *)jl_scratch(ctx, 1, (size_t)m * n * 4);
     float *das = nullptr;
     if (!da || !dr) return JL_ERR_OOM;
-    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(da, a, a_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    JL_CUDA_CHECK(ctx, cudaMemcpy2DAsync(da, (size_t)kp * esz, (const char *)a + (size_t)a_col_off * esz, (size_t)lda * esz,
+                                         (size_t)k * esz, m, cudaMemcpyHostToDevice, ctx->stream));
     if (a_dtype == JL_I8) {
-        das = (float *)jl_scratch(ctx, 2, (size_t)m * (lda / 32) * 4);
+        das = (float *)jl_scratch(ctx, 2, (size_t)m * (kp / 32) * 4);
         if (!das) return JL_ERR_OOM;
-        JL_CUDA_CHECK(ctx, cudaMemcpyAsync(das, a_scales, (size_t)m * (lda / 32) * 4, cudaMemcpyHostToDevice, ctx->stream));
+        JL_CUDA_CHECK(ctx, cudaMemcpy2DAsync(das, (size_t)(kp / 32) * 4, a_scales + a_col_off / 32, (size_t)(lda / 32) * 4,
+                                             (size_t)(k / 32) * 4, m, cudaMemcpyHostToDevice, ctx->stream));
     }
     const int pro = a_dtype == JL_I8 ? PRO_Q8_GLOBAL : (a_dtype == JL_BF16 ? PRO_BF16_GLOBAL : PRO_F32);
     const int chunk = jl_gemv_max_m(B.dtype, pro, k);
@@ -246,10 +252,10 @@ static int gemm_locked(jl_ctx *ctx, int a_dtype, const void *a, const float *a_s
         p.w_col_off = b_col_off;
         p.K = k;
         p.M = mc;
-        p.a = (const char *)da + (size_t)m0 * lda * esz;
-        p.a_scales = das ? das + (size_t)m0 * (lda / 32) : nullptr;
-        p.lda = lda;
-        p.a_col_off = a_col_off;
+        p.a = (const char *)da + (size_t)m0 * kp * esz;
+        p.a_scales = das ? das + (size_t)m0 * (kp / 32) : nullptr;
+        p.lda = kp;
+        p.a_col_off = 0;
         p.row0 = n0;
         p.total_rows = n;
         int rc = jl_launch_gemv(ctx, ctx->stream, p, pro, EPI_STORE);

@@ -53,7 +53,8 @@ def quantize_q4(x):
         iscale = np.where(scale != 0, np.float32(1.0) / scale, np.float32(0.0)).astype(np.float32)
         f = (b * iscale[..., None]).astype(np.float32) + np.float32(8.5)
         f = np.where(np.isnan(f), np.float32(0), f)
-        qi = np.clip(np.trunc(f), -2147483648.0, 2147483647.0).astype(np.int64)  # (int) saturates
+        # (int) saturates: clipped in double, where 2^31 - 1 is exact (in float it rounds to 2^31, which would wrap to 0, not -1)
+        qi = np.clip(np.trunc(f.astype(np.float64)), -2147483648.0, 2147483647.0).astype(np.int64)
     qi = ((qi + 128) % 256 - 128)  # (byte) wraps
     qi = np.minimum(qi, 15)
     lo = qi[..., :16] & 0xFF
@@ -103,7 +104,8 @@ def quantize_q8_activations(x, offset=0, length=None):
         d = (mx / np.float32(127.0)).astype(np.float32)
         idv = np.where(mx != 0, np.float32(127.0) / mx, np.float32(0.0)).astype(np.float32)
         f = ((b * idv[..., None]).astype(np.float32) + np.float32(0.5)).astype(np.float32)
-    qi = np.trunc(f).astype(np.int64)
+    # F2B narrows through int: NaN -> 0, (int) saturates (an infinite x * id, from a block of subnormals, becomes -1 or 0)
+    qi = np.where(np.isnan(f), 0.0, np.clip(np.trunc(f.astype(np.float64)), -2147483648.0, 2147483647.0)).astype(np.int64)
     qi = (qi + 128) % 256 - 128
     q[:, offset:offset + length] = qi.reshape(rows, length).astype(np.int8)
     s[:, offset // BLOCK:(offset + length) // BLOCK] = d
