@@ -1657,82 +1657,137 @@ static int run_decode(jl_model *m, int n, int max_pos, bool resident, bool want_
     return JL_OK;
 }
 
-// rows of m->logits / m->d_next with temperature != 0 (temperatures nullable): the reference's prefix-sum rule (AbstractModel.java:475-489)
-// replaces the arg-max; the logits rows are turned into exponentials in place, or, with `keep_logits`, in the top-k / top-p scratch rows
-// (`skip`, nullable: rows the top-k / top-p kernel has sampled; `src`: the rows to sample, m->logits or the processed rows of the
-// penalty kernel)
-static int sample_temperature_rows(jl_model *m, int n, const float *temperatures, const float *uniforms, const char *skip, bool keep_logits,
-                                   float *src) {
-    jl_ctx *ctx = m->ctx;
-    const size_t V = m->cfg.vocab_size;
-    for (int i = 0; temperatures && i < n; i++) {
-        if (temperatures[i] == 0.0f) continue; // :471-473 short-circuit: the arg-max stands
-        if (skip && skip[i]) continue;
+// One selection call: its nullable per-row inputs (HOST [n] each) and, after select_check, what they imply.  `topkp` and `logprobs` mark
+// the entry points that take those arguments (the *_constrained ones are topkp calls); the plain entry points skip the top-k / top-p
+// checks, so a negative temperature reaches the reference rule there.  Penalties (DESIGN §3.14) and masks (DESIGN §3.18) are on when
+// `pen` / `allow_row` are set; a call without a penalised or constrained row runs exactly as the narrower call.
+struct Selection {
+    const float *temperatures = nullptr, *uniforms = nullptr;
+    bool topkp = false;
+    const int32_t *top_k = nullptr;
+    const float *top_p = nullptr;
+    bool logprobs = false;
+    const int32_t *top_n = nullptr; // nullable = all -1
+    float *lp = nullptr;            // logprob outputs, each nullable
+    int32_t *ids = nullptr;
+    float *tlp = nullptr;
+    const jl_penalties *pen = nullptr;
+    int n_allow = 0;
+    const uint32_t *allow = nullptr;    // [n_allow][words]
+    const int32_t *allow_row = nullptr; // -1 = unconstrained
+    // derived by select_check
+    bool sampled = false;       // a row with temperature != 0
+    std::vector<char> filtered; // [n], topkp calls only: the rows the top-k / top-p kernel draws
+    int n_filtered = 0;
+    int n_lp = 0; // rows with top_n >= 0
+    PenaltyPlan plan;
+    int n_con = 0; // constrained rows
+    bool processed() const { return plan.n_on > 0 || n_con > 0; }
+    // the table of the processed rows: the penalties' own, or one unpenalised PenaltyRow per row for a call with masks only
+    size_t tab_bytes(int n) const { return pen ? plan.bytes : (size_t)n * sizeof(PenaltyRow); }
+};
+
+// The checks of one selection call, before any device work: uniforms for the sampled rows, top-k / top-p, logprobs, penalties, masks.
+// Logprobs, penalties and masks are refused under tensor parallelism (`tp`).  A constrained row with temperature > 0 then joins the
+// filtered rows: the top-k / top-p kernel draws it (its integer rule gives a banned token weight 0 and never draws one), whatever its
+// filter.
+static int select_check(jl_ctx *ctx, const char *who, int n, int vocab, bool tp, Selection &s) {
+    s.sampled = false, s.n_filtered = s.n_lp = s.n_con = 0, s.plan = PenaltyPlan();
+    for (int i = 0; s.temperatures && i < n; i++) s.sampled = s.sampled || s.temperatures[i] != 0.0f;
+    if (s.sampled && !s.uniforms) return jl_set_error(ctx, JL_ERR_INVALID, "%s: temperatures without uniform samples", who);
+    if (s.topkp) {
+        s.filtered.assign((size_t)n, 0);
+        M_CHECK(jl_topkp_check(ctx, who, n, vocab, s.temperatures, s.top_k, s.top_p, s.uniforms, s.filtered.data(), &s.n_filtered));
+    }
+    if (s.logprobs) {
+        if (tp) return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "%s: logprobs under tensor parallelism", who);
+        M_CHECK(jl_logprobs_check(ctx, who, n, vocab, s.top_n, &s.n_lp));
+    }
+    if (s.pen) {
+        if (tp) return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "%s: penalties under tensor parallelism", who);
+        M_CHECK(jl_penalty_check(ctx, who, n, vocab, s.pen, &s.plan));
+    }
+    if (!s.allow_row) return JL_OK;
+    if (tp) return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "%s: constrained rows under tensor parallelism", who);
+    M_CHECK(jl_constraint_check(ctx, who, n, vocab, s.n_allow, s.allow, s.allow_row, &s.n_con));
+    for (int i = 0; i < n; i++) {
+        if (s.allow_row[i] < 0 || !s.temperatures || !(s.temperatures[i] > 0.0f) || s.filtered[(size_t)i]) continue;
+        if (!(s.uniforms[i] >= 0.0f && s.uniforms[i] <= 1.0f))
+            return jl_set_error(ctx, JL_ERR_INVALID, "%s: row %d: uniform %g (in [0, 1])", who, i, (double)s.uniforms[i]);
+        if (vocab > JL_TOPKP_MAX_VOCAB) return jl_set_error(ctx, JL_ERR_INVALID, "%s: vocabulary of %d above %d", who, vocab, JL_TOPKP_MAX_VOCAB);
+        s.filtered[(size_t)i] = 1, s.n_filtered++;
+    }
+    return JL_OK;
+}
+
+// The buffers of one selection pass, DEVICE unless h_: proc, cnt (zero, and left zero), bias and ex hold n rows of vocab words; the
+// tables hold the call's; next holds the arg-max of the raw rows on entry and the tokens on return.
+struct SelectBufs {
+    float *proc;
+    unsigned *cnt;
+    float *bias;
+    void *d_tab, *h_tab;
+    uint32_t *d_mask, *h_mask;
+    TopkpRow *d_topkp, *h_topkp;
+    float *ex;
+    int32_t *next;
+    void *argmax;
+};
+
+// The selection of a checked call on `rows` (DEVICE [n][vocab]): penalties and masks turn them into the processed rows (two launches,
+// one without a penalised row) and the arg-max runs again on those; the filtered rows are drawn in one launch of the top-k / top-p
+// kernel, the other sampled rows by the reference's prefix-sum rule (AbstractModel.java:475-489), whose exponentials overwrite their
+// row unless the logprobs still read the raw rows.  The tables ride the stream, one copy each.
+static int select_pass(jl_ctx *ctx, cudaStream_t st, int n, int V, float *rows, const Selection &s, const SelectBufs &b) {
+    float *src = rows;
+    if (s.processed()) {
+        const jl_penalties none = {};
+        jl_penalty_pack(s.pen ? s.pen : &none, n, s.plan, b.h_tab);
+        const uint32_t *mask = nullptr;
+        if (s.n_con > 0) {
+            const int mr = jl_constraint_pack(n, V, s.n_allow, s.allow, s.allow_row, b.h_tab, b.h_mask);
+            JL_CUDA_CHECK(ctx, cudaMemcpyAsync(b.d_mask, b.h_mask, (size_t)mr * ((V + 31) / 32) * 4, cudaMemcpyHostToDevice, st));
+            mask = b.d_mask;
+        }
+        JL_CUDA_CHECK(ctx, cudaMemcpyAsync(b.d_tab, b.h_tab, s.tab_bytes(n), cudaMemcpyHostToDevice, st));
+        M_CHECK(jl_launch_penalties(ctx, st, rows, V, V, n, b.d_tab, s.plan, b.cnt, b.bias, mask, b.proc));
+        M_CHECK(jl_launch_argmax(ctx, st, b.proc, n, V, V, b.next, b.argmax));
+        src = b.proc;
+    }
+    if (s.n_filtered > 0) {
+        int c = 0;
+        for (int i = 0; i < n; i++)
+            if (s.filtered[(size_t)i])
+                b.h_topkp[c++] = TopkpRow{i, s.temperatures[i], s.top_k ? s.top_k[i] : 0, s.top_p ? s.top_p[i] : 1.0f, s.uniforms[i]};
+        JL_CUDA_CHECK(ctx, cudaMemcpyAsync(b.d_topkp, b.h_topkp, (size_t)c * sizeof(TopkpRow), cudaMemcpyHostToDevice, st));
+        M_CHECK(jl_launch_sample_topkp(ctx, st, src, V, V, b.d_topkp, c, b.ex, b.next));
+    }
+    for (int i = 0; s.sampled && i < n; i++) {
+        if (s.temperatures[i] == 0.0f) continue; // :471-473 short-circuit: the arg-max stands
+        if (s.n_filtered > 0 && s.filtered[(size_t)i]) continue;
         float *row = src + (size_t)i * V;
-        softmax_sample_kernel<<<1, 256, 0, m->stream>>>(row, keep_logits ? m->topkp_ex + (size_t)i * V : row, m->cfg.vocab_size, temperatures[i],
-                                                        uniforms[i], m->d_next + i);
+        softmax_sample_kernel<<<1, 256, 0, st>>>(row, s.n_lp > 0 ? b.ex + (size_t)i * V : row, V, s.temperatures[i], s.uniforms[i], b.next + i);
         ctx->launches++;
         JL_CUDA_CHECK(ctx, cudaGetLastError());
     }
     return JL_OK;
 }
 
-// Per-row top-k / top-p of one call (the *_topkp entry points).  `on` is false for the reference-rule entry points, which skip the
-// checks and the kernel entirely.
-struct TopkpArgs {
-    bool on = false;
-    const int32_t *top_k = nullptr;
-    const float *top_p = nullptr;
-    std::vector<char> filtered; // [n]: rows the top-k / top-p kernel samples
-    int n_filtered = 0;
-};
-
-static int topkp_check(jl_model *m, const char *who, int n, const float *temperatures, const float *uniforms, TopkpArgs &f) {
-    if (!f.on) return JL_OK;
-    f.filtered.assign((size_t)n, 0);
-    return jl_topkp_check(m->ctx, who, n, m->cfg.vocab_size, temperatures, f.top_k, f.top_p, uniforms, f.filtered.data(), &f.n_filtered);
-}
-
-// the filtered rows of `src` (m->logits or the processed rows) -> m->d_next, all in one launch of the top-k / top-p kernel (the rows
-// stay as they are)
-static int sample_filtered_rows(jl_model *m, int n, const float *temperatures, const float *uniforms, const TopkpArgs &f, const float *src) {
-    if (f.n_filtered == 0) return JL_OK;
+// the model's buffers of a call with processed rows and a penalty table of `tab` bytes, with `masks` the mask rows too (model lock
+// held).  The count words are zeroed in stream order.
+static int select_alloc(jl_model *m, size_t tab, bool masks) {
     jl_ctx *ctx = m->ctx;
-    int c = 0;
-    for (int i = 0; i < n; i++)
-        if (f.filtered[(size_t)i])
-            m->h_topkp[c++] = TopkpRow{i, temperatures[i], f.top_k ? f.top_k[i] : 0, f.top_p ? f.top_p[i] : 1.0f, uniforms[i]};
-    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(m->d_topkp, m->h_topkp, (size_t)c * sizeof(TopkpRow), cudaMemcpyHostToDevice, m->stream));
-    return jl_launch_sample_topkp(ctx, m->stream, src, m->cfg.vocab_size, m->cfg.vocab_size, m->d_topkp, c, m->topkp_ex, m->d_next);
-}
-
-// Penalties of one call (the *_penalized entry points; DESIGN §3.14): `pen` nullable; a call without a penalised row runs exactly as
-// the matching _logprobs call.
-struct PenaltyArgs {
-    const jl_penalties *pen = nullptr;
-    PenaltyPlan plan;
-};
-
-static int penalty_check(jl_model *m, const char *who, int n, PenaltyArgs &a) {
-    if (!a.pen) return JL_OK;
-    if (m->cfg.tp_size > 1) return jl_set_error(m->ctx, JL_ERR_UNSUPPORTED, "%s: penalties under tensor parallelism", who);
-    return jl_penalty_check(m->ctx, who, n, m->cfg.vocab_size, a.pen, &a.plan);
-}
-
-// the penalty buffers for a call with a penalised row and a table of `bytes` (model lock held)
-static int penalty_alloc(jl_model *m, size_t bytes) {
-    jl_ctx *ctx = m->ctx;
+    const int S = m->cfg.max_sessions, rows = S < JL_MAX_DECODE_ROWS ? S : JL_MAX_DECODE_ROWS;
     if (!m->pen_out) {
-        const int S = m->cfg.max_sessions, rows = S < JL_MAX_DECODE_ROWS ? S : JL_MAX_DECODE_ROWS;
         const size_t rb = (size_t)rows * m->cfg.vocab_size * 4;
         M_CHECK(dev_alloc(ctx, (void **)&m->pen_out, rb));
         M_CHECK(dev_alloc(ctx, (void **)&m->pen_bias, rb));
         M_CHECK(dev_alloc(ctx, (void **)&m->pen_cnt, rb));
-        JL_CUDA_CHECK(ctx, cudaMemset(m->pen_cnt, 0, rb));
+        JL_CUDA_CHECK(ctx, cudaMemsetAsync(m->pen_cnt, 0, rb, m->stream));
     }
-    if (bytes > m->pen_tab_cap) {
+    if (tab > m->pen_tab_cap) {
         size_t cap = 4096;
-        while (cap < bytes) cap *= 2;
+        while (cap < tab) cap *= 2;
         if (m->d_pen_tab) cudaFree(m->d_pen_tab), m->d_pen_tab = nullptr;
         if (m->h_pen_tab) cudaFreeHost(m->h_pen_tab), m->h_pen_tab = nullptr;
         m->pen_tab_cap = 0;
@@ -1740,142 +1795,54 @@ static int penalty_alloc(jl_model *m, size_t bytes) {
         JL_CUDA_CHECK(ctx, cudaMallocHost(&m->h_pen_tab, cap));
         m->pen_tab_cap = cap;
     }
-    return JL_OK;
-}
-
-// Allowed-token masks of one call (the *_constrained entry points; DESIGN §3.18): allow_row nullable; a call without a constrained row
-// runs exactly as the matching _penalized call.
-struct ConstraintArgs {
-    int n_allow = 0;
-    const uint32_t *allow = nullptr;   // HOST [n_allow][words]
-    const int32_t *allow_row = nullptr; // HOST [n], -1 = unconstrained
-    int n_on = 0;                       // constrained rows
-};
-
-// after topkp_check: a constrained row with temperature > 0 is drawn by the top-k / top-p kernel (the integer rule gives a banned
-// token weight 0 and never draws one), whatever its filter
-static int constraint_check(jl_model *m, const char *who, int n, const float *temperatures, const float *uniforms, TopkpArgs &f,
-                            ConstraintArgs &a) {
-    if (!a.allow_row) return JL_OK;
-    jl_ctx *ctx = m->ctx;
-    if (m->cfg.tp_size > 1) return jl_set_error(ctx, JL_ERR_UNSUPPORTED, "%s: constrained rows under tensor parallelism", who);
-    M_CHECK(jl_constraint_check(ctx, who, n, m->cfg.vocab_size, a.n_allow, a.allow, a.allow_row, &a.n_on));
-    for (int i = 0; i < n; i++) {
-        if (a.allow_row[i] < 0 || !temperatures || !(temperatures[i] > 0.0f) || f.filtered[(size_t)i]) continue;
-        if (!(uniforms[i] >= 0.0f && uniforms[i] <= 1.0f))
-            return jl_set_error(ctx, JL_ERR_INVALID, "%s: row %d: uniform %g (in [0, 1])", who, i, (double)uniforms[i]);
-        if (m->cfg.vocab_size > JL_TOPKP_MAX_VOCAB)
-            return jl_set_error(ctx, JL_ERR_INVALID, "%s: vocabulary of %d above %d", who, m->cfg.vocab_size, JL_TOPKP_MAX_VOCAB);
-        f.filtered[(size_t)i] = 1, f.n_filtered++;
+    if (masks && !m->d_mask) {
+        const size_t bytes = (size_t)rows * ((m->cfg.vocab_size + 31) / 32) * 4;
+        M_CHECK(dev_alloc(ctx, (void **)&m->d_mask, bytes));
+        JL_CUDA_CHECK(ctx, cudaMallocHost((void **)&m->h_mask, bytes));
     }
     return JL_OK;
 }
 
-// the mask buffers for a call with a constrained row (model lock held)
-static int constraint_alloc(jl_model *m) {
-    if (m->d_mask) return JL_OK;
-    jl_ctx *ctx = m->ctx;
-    const int S = m->cfg.max_sessions, rows = S < JL_MAX_DECODE_ROWS ? S : JL_MAX_DECODE_ROWS;
-    const size_t bytes = (size_t)rows * ((m->cfg.vocab_size + 31) / 32) * 4;
-    M_CHECK(dev_alloc(ctx, (void **)&m->d_mask, bytes));
-    JL_CUDA_CHECK(ctx, cudaMallocHost((void **)&m->h_mask, bytes));
-    return JL_OK;
-}
-
-// the table of a call's processed rows: the penalties' own, or one unpenalised PenaltyRow per row for a call with masks only
-static size_t processed_tab_bytes(int n, const PenaltyArgs &a) { return a.pen ? a.plan.bytes : (size_t)n * sizeof(PenaltyRow); }
-
-// after the logits_out copy: m->logits -> the processed rows m->pen_out (penalties, then masks; two launches, one without a penalised
-// row), then the arg-max of every row again on those (the greedy tokens of the decode graphs and the persistent kernel were taken on
-// the raw rows).  The table and the mask rows ride the stream, one copy each.
-static int penalty_rows(jl_model *m, int n, const PenaltyArgs &a, const ConstraintArgs &c) {
+// Everything after the logits of a checked call (m->logits, n rows, their arg-max in m->d_next; model lock held): logits_out gets the raw
+// logits before any row is exponentiated, then the selection pass, one logprob launch for the rows with top_n >= 0 (of the raw logits,
+// the chosen tokens as targets), and the tokens.  `decode`: the step's end event is recorded, and the persistent kernel's status checked
+// after the synchronise.
+static int select_tail(jl_model *m, int n, Selection &s, float *logits_out, int32_t *tokens_out, bool decode) {
     jl_ctx *ctx = m->ctx;
     const int V = m->cfg.vocab_size;
-    const jl_penalties none = {};
-    jl_penalty_pack(a.pen ? a.pen : &none, n, a.plan, m->h_pen_tab);
-    const uint32_t *mask = nullptr;
-    if (c.n_on > 0) {
-        const int rows = jl_constraint_pack(n, V, c.n_allow, c.allow, c.allow_row, m->h_pen_tab, m->h_mask);
-        JL_CUDA_CHECK(ctx, cudaMemcpyAsync(m->d_mask, m->h_mask, (size_t)rows * ((V + 31) / 32) * 4, cudaMemcpyHostToDevice, m->stream));
-        mask = m->d_mask;
+    if (logits_out) JL_CUDA_CHECK(ctx, cudaMemcpyAsync(logits_out, m->logits, (size_t)n * V * 4, cudaMemcpyDeviceToHost, m->stream));
+    if (s.processed()) M_CHECK(select_alloc(m, s.tab_bytes(n), s.n_con > 0));
+    const SelectBufs b{m->pen_out, m->pen_cnt, m->pen_bias, m->d_pen_tab, m->h_pen_tab, m->d_mask, m->h_mask,
+                       m->d_topkp, m->h_topkp, m->topkp_ex, m->d_next, m->argmax_scratch};
+    M_CHECK(select_pass(ctx, m->stream, n, V, m->logits, s, b));
+    jl_model::LpBufs &lb = m->lp;
+    if (s.n_lp > 0) {
+        int c = 0;
+        for (int i = 0; i < n; i++)
+            if (s.top_n[i] >= 0) lb.h_rows[c++] = LogprobRow{i, s.top_n[i]};
+        JL_CUDA_CHECK(ctx, cudaMemcpyAsync(lb.d_rows, lb.h_rows, (size_t)c * sizeof(LogprobRow), cudaMemcpyHostToDevice, m->stream));
+        M_CHECK(jl_launch_logprobs(ctx, m->stream, m->logits, V, V, lb.d_rows, c, m->d_next, lb.ws, lb.cnt, lb.d_out));
+        JL_CUDA_CHECK(ctx, cudaMemcpyAsync(lb.h_out, lb.d_out, (size_t)n * sizeof(LogprobOut), cudaMemcpyDeviceToHost, m->stream));
     }
-    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(m->d_pen_tab, m->h_pen_tab, processed_tab_bytes(n, a), cudaMemcpyHostToDevice, m->stream));
-    M_CHECK(jl_launch_penalties(ctx, m->stream, m->logits, V, V, n, m->d_pen_tab, a.plan, m->pen_cnt, m->pen_bias, mask, m->pen_out));
-    return jl_launch_argmax(ctx, m->stream, m->pen_out, n, V, V, m->d_next, m->argmax_scratch);
-}
-
-// everything after the logits of one call: penalties and masks, top-k / top-p rows, reference-rule rows, logprobs (of the raw logits)
-static int select_rows(jl_model *m, int n, const float *temperatures, const float *uniforms, bool sampled, const TopkpArgs &f, int lp_on,
-                       const PenaltyArgs &pa, const ConstraintArgs &ca) {
-    float *src = m->logits;
-    if (pa.plan.n_on > 0 || ca.n_on > 0) {
-        M_CHECK(penalty_rows(m, n, pa, ca));
-        src = m->pen_out;
-    }
-    M_CHECK(sample_filtered_rows(m, n, temperatures, uniforms, f, src));
-    if (sampled) M_CHECK(sample_temperature_rows(m, n, temperatures, uniforms, f.on ? f.filtered.data() : nullptr, lp_on > 0, src));
+    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(pinned_next(m), m->d_next, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
+    if (decode) JL_CUDA_CHECK(ctx, cudaEventRecord(m->ev_end, m->stream));
+    JL_CUDA_CHECK(ctx, cudaStreamSynchronize(m->stream));
+    if (decode && n == 1 && use_pd(m)) M_CHECK(pd_check(m));
+    memcpy(tokens_out, pinned_next(m), (size_t)n * 4);
+    if (s.logprobs) jl_logprobs_unpack(lb.h_out, s.top_n, n, s.lp, s.ids, s.tlp);
     return JL_OK;
 }
 
-// Per-row logprobs of one call (the *_logprobs entry points; DESIGN §3.13).  `on` is false for every other entry point; a call whose
-// rows all have top_n -1 runs exactly as the matching _topkp call.
-struct LogprobArgs {
-    bool on = false;
-    const int32_t *top_n = nullptr; // [n], nullable = all -1
-    float *lp = nullptr;            // HOST outputs, each nullable
-    int32_t *ids = nullptr;
-    float *tlp = nullptr;
-    int n_on = 0; // rows with top_n >= 0
-};
-
-static int logprobs_check(jl_model *m, const char *who, int n, LogprobArgs &a) {
-    if (!a.on) return JL_OK;
-    if (m->cfg.tp_size > 1) return jl_set_error(m->ctx, JL_ERR_UNSUPPORTED, "%s: logprobs under tensor parallelism", who);
-    return jl_logprobs_check(m->ctx, who, n, m->cfg.vocab_size, a.top_n, &a.n_on);
-}
-
-// after the sampling kernels: one logprob launch for the rows with top_n >= 0 of m->logits (still raw: the draws wrote their
-// exponentials to scratch rows), the chosen tokens m->d_next as targets; the outputs are copied to the pinned staging in stream order
-static int logprob_rows(jl_model *m, int n, const LogprobArgs &a) {
-    if (a.n_on == 0) return JL_OK;
-    jl_ctx *ctx = m->ctx;
-    jl_model::LpBufs &b = m->lp;
-    int c = 0;
-    for (int i = 0; i < n; i++)
-        if (a.top_n[i] >= 0) b.h_rows[c++] = LogprobRow{i, a.top_n[i]};
-    const int V = m->cfg.vocab_size;
-    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(b.d_rows, b.h_rows, (size_t)c * sizeof(LogprobRow), cudaMemcpyHostToDevice, m->stream));
-    M_CHECK(jl_launch_logprobs(ctx, m->stream, m->logits, V, V, b.d_rows, c, m->d_next, b.ws, b.cnt, b.d_out));
-    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(b.h_out, b.d_out, (size_t)n * sizeof(LogprobOut), cudaMemcpyDeviceToHost, m->stream));
-    return JL_OK;
-}
-
-// after the synchronise: the staged outputs -> the caller's arrays
-static void logprob_unpack(jl_model *m, int n, const LogprobArgs &a) {
-    if (a.on) jl_logprobs_unpack(m->lp.h_out, a.top_n, n, a.lp, a.ids, a.tlp);
-}
-
-// temperatures / uniforms: nullable [n]; a row with temperature != 0 is sampled with the reference's prefix-sum rule
-// (AbstractModel.java:475-489, softmax_sample_kernel) from its logits row instead of taking the arg-max, or by the top-k / top-p kernel
-// when `f` filters it.  `lp`: logprobs of the chosen tokens.  `pa`: penalties; the selection of every row then reads its processed row.
-static int decode_impl(jl_model *m, int n, const int32_t *sessions, const int32_t *tokens, const int32_t *positions,
-                       const float *temperatures, const float *uniforms, int32_t *next_tokens, float *logits_out, TopkpArgs &&f = TopkpArgs(),
-                       LogprobArgs lp = LogprobArgs(), PenaltyArgs pa = PenaltyArgs(), ConstraintArgs ca = ConstraintArgs()) {
+// One decode step of n sessions; `s` selects each row's token from its logits row: the arg-max, or a draw (see Selection).
+static int decode_impl(jl_model *m, int n, const int32_t *sessions, const int32_t *tokens, const int32_t *positions, int32_t *next_tokens,
+                       float *logits_out, Selection &s) {
     if (!m || !m->finalized || n <= 0 || n > m->cfg.max_sessions || n > JL_MAX_DECODE_ROWS || !sessions || !tokens || !positions ||
         !next_tokens)
         return m ? jl_set_error(m->ctx, JL_ERR_INVALID, "decode: bad arguments (n=%d, max %d)", n, JL_MAX_DECODE_ROWS) : JL_ERR_INVALID;
-    bool sampled = false;
-    for (int i = 0; temperatures && i < n; i++) sampled = sampled || temperatures[i] != 0.0f;
-    if (sampled && !uniforms) return jl_set_error(m->ctx, JL_ERR_INVALID, "decode: temperatures without uniform samples");
-    M_CHECK(topkp_check(m, "decode", n, temperatures, uniforms, f));
-    M_CHECK(logprobs_check(m, "decode", n, lp));
-    M_CHECK(penalty_check(m, "decode", n, pa));
-    M_CHECK(constraint_check(m, "decode", n, temperatures, uniforms, f, ca));
+    M_CHECK(select_check(m->ctx, "decode", n, m->cfg.vocab_size, m->cfg.tp_size > 1, s));
     std::lock_guard<std::recursive_mutex> model_lock(m->mu);
     jl_ctx *ctx = m->ctx;
     JL_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
-    if (pa.plan.n_on > 0 || ca.n_on > 0) M_CHECK(penalty_alloc(m, processed_tab_bytes(n, pa)));
-    if (ca.n_on > 0) M_CHECK(constraint_alloc(m));
     int max_pos = 0;
     for (int i = 0; i < n; i++) {
         if (sessions[i] < 0 || sessions[i] >= m->cfg.max_sessions || positions[i] < 0)
@@ -1887,17 +1854,8 @@ static int decode_impl(jl_model *m, int n, const int32_t *sessions, const int32_
     }
     JL_CUDA_CHECK(ctx, cudaEventRecord(m->ev_begin, m->stream));
     M_CHECK(stage_rows(m, n, tokens, positions, sessions));
-    M_CHECK(run_decode(m, n, max_pos, false, logits_out != nullptr || sampled || pa.plan.n_on > 0 || ca.n_on > 0));
-    if (logits_out) // before the sampling kernels turn the sampled rows into exponentials in place
-        JL_CUDA_CHECK(ctx, cudaMemcpyAsync(logits_out, m->logits, (size_t)n * m->cfg.vocab_size * 4, cudaMemcpyDeviceToHost, m->stream));
-    M_CHECK(select_rows(m, n, temperatures, uniforms, sampled, f, lp.n_on, pa, ca));
-    M_CHECK(logprob_rows(m, n, lp));
-    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(pinned_next(m), m->d_next, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
-    JL_CUDA_CHECK(ctx, cudaEventRecord(m->ev_end, m->stream));
-    JL_CUDA_CHECK(ctx, cudaStreamSynchronize(m->stream));
-    if (n == 1 && use_pd(m)) M_CHECK(pd_check(m));
-    memcpy(next_tokens, pinned_next(m), (size_t)n * 4);
-    logprob_unpack(m, n, lp);
+    M_CHECK(run_decode(m, n, max_pos, false, logits_out != nullptr || s.sampled || s.processed()));
+    M_CHECK(select_tail(m, n, s, logits_out, next_tokens, true));
     float ms = 0;
     cudaEventElapsedTime(&ms, m->ev_begin, m->ev_end);
     m->last_total_ms = ms;
@@ -1906,136 +1864,97 @@ static int decode_impl(jl_model *m, int n, const int32_t *sessions, const int32_
 
 // AbstractModel.sample on the last forwarded rows of n distinct sessions (arguments already checked): the rows are gathered in one
 // launch and share one lm_head pass (sample_rows' wide mode: one weight pass for 9..64 rows).  logits_out gets the raw logits.
-static int sample_sessions(jl_model *m, int n, const int32_t *sessions, const float *temperatures, const float *uniforms,
-                           int32_t *tokens_out, float *logits_out, const TopkpArgs &f = TopkpArgs(), const LogprobArgs &lp = LogprobArgs(),
-                           const PenaltyArgs &pa = PenaltyArgs(), const ConstraintArgs &ca = ConstraintArgs()) {
+static int sample_sessions(jl_model *m, int n, const int32_t *sessions, int32_t *tokens_out, float *logits_out, Selection &s) {
     std::lock_guard<std::recursive_mutex> model_lock(m->mu);
     jl_ctx *ctx = m->ctx;
     JL_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
-    if (pa.plan.n_on > 0 || ca.n_on > 0) M_CHECK(penalty_alloc(m, processed_tab_bytes(n, pa)));
-    if (ca.n_on > 0) M_CHECK(constraint_alloc(m));
     memcpy(pinned_rows(m), sessions, (size_t)n * 4);
     JL_CUDA_CHECK(ctx, cudaMemcpyAsync(m->d_rows, pinned_rows(m), (size_t)n * 4, cudaMemcpyHostToDevice, m->stream));
     M_CHECK(copy_rows(m, m->xb, nullptr, m->last_hidden, m->d_rows, n));
     M_CHECK(sample_rows(m, m->xb, n));
-    if (logits_out) // before the sampled rows are exponentiated in place
-        JL_CUDA_CHECK(ctx, cudaMemcpyAsync(logits_out, m->logits, (size_t)n * m->cfg.vocab_size * 4, cudaMemcpyDeviceToHost, m->stream));
-    M_CHECK(select_rows(m, n, temperatures, uniforms, true, f, lp.n_on, pa, ca));
-    M_CHECK(logprob_rows(m, n, lp));
-    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(pinned_next(m), m->d_next, (size_t)n * 4, cudaMemcpyDeviceToHost, m->stream));
-    JL_CUDA_CHECK(ctx, cudaStreamSynchronize(m->stream));
-    memcpy(tokens_out, pinned_next(m), (size_t)n * 4);
-    logprob_unpack(m, n, lp);
-    return JL_OK;
+    return select_tail(m, n, s, logits_out, tokens_out, false);
 }
 
 extern "C" int jl_model_sample(jl_model *m, int session, float temperature, float uniform, int32_t *token_out,
                                float *logits_out) {
     if (!m || !m->finalized || !token_out || session < 0 || session >= m->cfg.max_sessions) return JL_ERR_INVALID;
+    Selection s{&temperature, &uniform};
+    M_CHECK(select_check(m->ctx, "sample", 1, m->cfg.vocab_size, m->cfg.tp_size > 1, s));
     // logits_out is written at temperature 0 only
-    return sample_sessions(m, 1, &session, &temperature, &uniform, token_out, temperature == 0.0f ? logits_out : nullptr);
+    return sample_sessions(m, 1, &session, token_out, temperature == 0.0f ? logits_out : nullptr, s);
 }
 
-static int sample_multi_impl(jl_model *m, int n, const int32_t *sessions, const float *temperatures, const float *uniforms,
-                             int32_t *tokens_out, float *logits_out, TopkpArgs &&f = TopkpArgs(), LogprobArgs lp = LogprobArgs(),
-                             PenaltyArgs pa = PenaltyArgs(), ConstraintArgs ca = ConstraintArgs()) {
+static int sample_multi_impl(jl_model *m, int n, const int32_t *sessions, int32_t *tokens_out, float *logits_out, Selection &s) {
     if (!m || !m->finalized) return JL_ERR_INVALID;
     jl_ctx *ctx = m->ctx;
     const int S = m->cfg.max_sessions, cap = S < JL_MAX_DECODE_ROWS ? S : JL_MAX_DECODE_ROWS;
     if (!sessions || !tokens_out) return jl_set_error(ctx, JL_ERR_INVALID, "sample_multi: null argument");
     if (n < 1 || n > cap) return jl_set_error(ctx, JL_ERR_INVALID, "sample_multi: %d rows (1..%d)", n, cap);
     std::vector<char> seen((size_t)S, 0);
-    bool sampled = false;
     for (int i = 0; i < n; i++) {
         if (sessions[i] < 0 || sessions[i] >= S) return jl_set_error(ctx, JL_ERR_INVALID, "sample_multi: session %d out of range", sessions[i]);
         if (seen[(size_t)sessions[i]]) return jl_set_error(ctx, JL_ERR_INVALID, "sample_multi: session %d appears twice", sessions[i]);
         seen[(size_t)sessions[i]] = 1;
-        sampled = sampled || (temperatures && temperatures[i] != 0.0f);
     }
-    if (sampled && !uniforms) return jl_set_error(ctx, JL_ERR_INVALID, "sample_multi: temperatures without uniform samples");
-    M_CHECK(topkp_check(m, "sample_multi", n, temperatures, uniforms, f));
-    M_CHECK(logprobs_check(m, "sample_multi", n, lp));
-    M_CHECK(penalty_check(m, "sample_multi", n, pa));
-    M_CHECK(constraint_check(m, "sample_multi", n, temperatures, uniforms, f, ca));
-    return sample_sessions(m, n, sessions, temperatures, uniforms, tokens_out, logits_out, f, lp, pa, ca);
+    M_CHECK(select_check(ctx, "sample_multi", n, m->cfg.vocab_size, m->cfg.tp_size > 1, s));
+    return sample_sessions(m, n, sessions, tokens_out, logits_out, s);
 }
 
 extern "C" int jl_model_sample_multi(jl_model *m, int n, const int32_t *sessions, const float *temperatures, const float *uniforms,
                                      int32_t *tokens_out, float *logits_out) {
-    return sample_multi_impl(m, n, sessions, temperatures, uniforms, tokens_out, logits_out);
-}
-
-static TopkpArgs topkp_args(const int32_t *top_k, const float *top_p) {
-    TopkpArgs f;
-    f.on = true, f.top_k = top_k, f.top_p = top_p;
-    return f;
+    Selection s{temperatures, uniforms};
+    return sample_multi_impl(m, n, sessions, tokens_out, logits_out, s);
 }
 
 extern "C" int jl_model_sample_multi_topkp(jl_model *m, int n, const int32_t *sessions, const float *temperatures, const int32_t *top_k,
                                            const float *top_p, const float *uniforms, int32_t *tokens_out, float *logits_out) {
-    return sample_multi_impl(m, n, sessions, temperatures, uniforms, tokens_out, logits_out, topkp_args(top_k, top_p));
+    Selection s{temperatures, uniforms, true, top_k, top_p};
+    return sample_multi_impl(m, n, sessions, tokens_out, logits_out, s);
 }
 
 extern "C" int jl_model_decode_sample_topkp(jl_model *m, int n, const int32_t *sessions, const int32_t *tokens, const int32_t *positions,
                                             const float *temperatures, const int32_t *top_k, const float *top_p, const float *uniforms,
                                             int32_t *next_tokens, float *logits_out) {
-    return decode_impl(m, n, sessions, tokens, positions, temperatures, uniforms, next_tokens, logits_out, topkp_args(top_k, top_p));
-}
-
-static LogprobArgs logprob_args(const int32_t *top_n, float *lp_out, int32_t *top_ids_out, float *top_lp_out) {
-    LogprobArgs a;
-    a.on = true, a.top_n = top_n, a.lp = lp_out, a.ids = top_ids_out, a.tlp = top_lp_out;
-    return a;
+    Selection s{temperatures, uniforms, true, top_k, top_p};
+    return decode_impl(m, n, sessions, tokens, positions, next_tokens, logits_out, s);
 }
 
 extern "C" int jl_model_sample_multi_logprobs(jl_model *m, int n, const int32_t *sessions, const float *temperatures, const int32_t *top_k,
                                               const float *top_p, const float *uniforms, const int32_t *top_n, int32_t *tokens_out, float *lp_out,
                                               int32_t *top_ids_out, float *top_lp_out, float *logits_out) {
-    return sample_multi_impl(m, n, sessions, temperatures, uniforms, tokens_out, logits_out, topkp_args(top_k, top_p),
-                             logprob_args(top_n, lp_out, top_ids_out, top_lp_out));
+    Selection s{temperatures, uniforms, true, top_k, top_p, true, top_n, lp_out, top_ids_out, top_lp_out};
+    return sample_multi_impl(m, n, sessions, tokens_out, logits_out, s);
 }
 
 extern "C" int jl_model_decode_logprobs(jl_model *m, int n, const int32_t *sessions, const int32_t *tokens, const int32_t *positions,
                                         const float *temperatures, const int32_t *top_k, const float *top_p, const float *uniforms,
                                         const int32_t *top_n, int32_t *next_tokens, float *lp_out, int32_t *top_ids_out, float *top_lp_out,
                                         float *logits_out) {
-    return decode_impl(m, n, sessions, tokens, positions, temperatures, uniforms, next_tokens, logits_out, topkp_args(top_k, top_p),
-                       logprob_args(top_n, lp_out, top_ids_out, top_lp_out));
-}
-
-static PenaltyArgs penalty_args(const jl_penalties *pen) {
-    PenaltyArgs a;
-    a.pen = pen;
-    return a;
+    Selection s{temperatures, uniforms, true, top_k, top_p, true, top_n, lp_out, top_ids_out, top_lp_out};
+    return decode_impl(m, n, sessions, tokens, positions, next_tokens, logits_out, s);
 }
 
 extern "C" int jl_model_sample_multi_penalized(jl_model *m, int n, const int32_t *sessions, const float *temperatures, const int32_t *top_k,
                                                const float *top_p, const float *uniforms, const int32_t *top_n, const jl_penalties *pen,
                                                int32_t *tokens_out, float *lp_out, int32_t *top_ids_out, float *top_lp_out, float *logits_out) {
-    return sample_multi_impl(m, n, sessions, temperatures, uniforms, tokens_out, logits_out, topkp_args(top_k, top_p),
-                             logprob_args(top_n, lp_out, top_ids_out, top_lp_out), penalty_args(pen));
+    Selection s{temperatures, uniforms, true, top_k, top_p, true, top_n, lp_out, top_ids_out, top_lp_out, pen};
+    return sample_multi_impl(m, n, sessions, tokens_out, logits_out, s);
 }
 
 extern "C" int jl_model_decode_penalized(jl_model *m, int n, const int32_t *sessions, const int32_t *tokens, const int32_t *positions,
                                          const float *temperatures, const int32_t *top_k, const float *top_p, const float *uniforms,
                                          const int32_t *top_n, const jl_penalties *pen, int32_t *next_tokens, float *lp_out, int32_t *top_ids_out,
                                          float *top_lp_out, float *logits_out) {
-    return decode_impl(m, n, sessions, tokens, positions, temperatures, uniforms, next_tokens, logits_out, topkp_args(top_k, top_p),
-                       logprob_args(top_n, lp_out, top_ids_out, top_lp_out), penalty_args(pen));
-}
-
-static ConstraintArgs constraint_args(int n_allow, const uint32_t *allow, const int32_t *allow_row) {
-    ConstraintArgs a;
-    a.n_allow = n_allow, a.allow = allow, a.allow_row = allow_row;
-    return a;
+    Selection s{temperatures, uniforms, true, top_k, top_p, true, top_n, lp_out, top_ids_out, top_lp_out, pen};
+    return decode_impl(m, n, sessions, tokens, positions, next_tokens, logits_out, s);
 }
 
 extern "C" int jl_model_sample_multi_constrained(jl_model *m, int n, const int32_t *sessions, const float *temperatures, const int32_t *top_k,
                                                  const float *top_p, const float *uniforms, const int32_t *top_n, const jl_penalties *pen,
                                                  int n_allow, const uint32_t *allow, const int32_t *allow_row, int32_t *tokens_out, float *lp_out,
                                                  int32_t *top_ids_out, float *top_lp_out, float *logits_out) {
-    return sample_multi_impl(m, n, sessions, temperatures, uniforms, tokens_out, logits_out, topkp_args(top_k, top_p),
-                             logprob_args(top_n, lp_out, top_ids_out, top_lp_out), penalty_args(pen), constraint_args(n_allow, allow, allow_row));
+    Selection s{temperatures, uniforms, true, top_k, top_p, true, top_n, lp_out, top_ids_out, top_lp_out, pen, n_allow, allow, allow_row};
+    return sample_multi_impl(m, n, sessions, tokens_out, logits_out, s);
 }
 
 extern "C" int jl_model_decode_constrained(jl_model *m, int n, const int32_t *sessions, const int32_t *tokens, const int32_t *positions,
@@ -2043,12 +1962,12 @@ extern "C" int jl_model_decode_constrained(jl_model *m, int n, const int32_t *se
                                            const int32_t *top_n, const jl_penalties *pen, int n_allow, const uint32_t *allow,
                                            const int32_t *allow_row, int32_t *next_tokens, float *lp_out, int32_t *top_ids_out,
                                            float *top_lp_out, float *logits_out) {
-    return decode_impl(m, n, sessions, tokens, positions, temperatures, uniforms, next_tokens, logits_out, topkp_args(top_k, top_p),
-                       logprob_args(top_n, lp_out, top_ids_out, top_lp_out), penalty_args(pen), constraint_args(n_allow, allow, allow_row));
+    Selection s{temperatures, uniforms, true, top_k, top_p, true, top_n, lp_out, top_ids_out, top_lp_out, pen, n_allow, allow, allow_row};
+    return decode_impl(m, n, sessions, tokens, positions, next_tokens, logits_out, s);
 }
 
-// HOST-buffer entry point for crafted rows: the selection of the model calls (penalties and masks into processed rows, the arg-max on
-// them, constrained and filtered sampled rows by the top-k / top-p kernel, the other sampled rows by the reference's rule)
+// HOST-buffer entry point for crafted rows: the model calls' selection pass (select_pass) on the rows, after the arg-max the model's
+// lm_head pass takes.  Every sampled row's uniform must lie in [0, 1].
 extern "C" int jl_select_constrained(jl_ctx *ctx, int n, int vocab, const float *logits, int64_t ld, const float *temperatures,
                                      const int32_t *top_k, const float *top_p, const float *uniforms, const jl_penalties *pen, int n_allow,
                                      const uint32_t *allow, const int32_t *allow_row, int32_t *out) {
@@ -2056,85 +1975,45 @@ extern "C" int jl_select_constrained(jl_ctx *ctx, int n, int vocab, const float 
     const char *who = "select_constrained";
     if (n < 1 || n > 65535 || vocab < 1 || vocab > JL_TOPKP_MAX_VOCAB || ld < vocab || !logits || !out)
         return jl_set_error(ctx, JL_ERR_INVALID, "%s: bad arguments (n=%d, vocab=%d, ld=%lld)", who, n, vocab, (long long)ld);
-    std::vector<char> filtered((size_t)n, 0);
-    int nf = 0;
-    M_CHECK(jl_topkp_check(ctx, who, n, vocab, temperatures, top_k, top_p, uniforms, filtered.data(), &nf));
-    PenaltyPlan plan;
-    M_CHECK(jl_penalty_check(ctx, who, n, vocab, pen, &plan));
-    int n_con = 0;
-    M_CHECK(jl_constraint_check(ctx, who, n, vocab, n_allow, allow, allow_row, &n_con));
-    for (int i = 0; i < n; i++) {
-        if (!temperatures || !(temperatures[i] > 0.0f)) continue;
-        if (!(uniforms[i] >= 0.0f && uniforms[i] <= 1.0f))
+    Selection s{temperatures, uniforms, true, top_k, top_p, false, nullptr, nullptr, nullptr, nullptr, pen, n_allow, allow, allow_row};
+    M_CHECK(select_check(ctx, who, n, vocab, false, s));
+    for (int i = 0; s.sampled && i < n; i++)
+        if (temperatures[i] > 0.0f && !(uniforms[i] >= 0.0f && uniforms[i] <= 1.0f))
             return jl_set_error(ctx, JL_ERR_INVALID, "%s: row %d: uniform %g (in [0, 1])", who, i, (double)uniforms[i]);
-        if (allow_row && allow_row[i] >= 0 && !filtered[(size_t)i]) filtered[(size_t)i] = 1, nf++;
-    }
-    const jl_penalties none = {};
-    const size_t words = (size_t)(vocab + 31) / 32;
-    std::vector<char> tab(pen ? plan.bytes : (size_t)n * sizeof(PenaltyRow));
-    jl_penalty_pack(pen ? pen : &none, n, plan, tab.data());
-    std::vector<uint32_t> mrows;
-    int nm = 0;
-    if (n_con > 0) {
-        mrows.resize((size_t)n * words);
-        nm = jl_constraint_pack(n, vocab, n_allow, allow, allow_row, tab.data(), mrows.data());
-    }
-    const bool processed = plan.n_on > 0 || n_con > 0;
+    std::vector<char> h_tab(s.processed() ? s.tab_bytes(n) : 0);
+    std::vector<uint32_t> h_mask(s.n_con > 0 ? (size_t)n * ((vocab + 31) / 32) : 0);
+    std::vector<TopkpRow> h_topkp((size_t)s.n_filtered);
     std::lock_guard<std::mutex> lk(ctx->mu);
     JL_CUDA_CHECK(ctx, cudaSetDevice(ctx->device));
     auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    const size_t lb = ((size_t)(n - 1) * ld + vocab) * 4, rb = al((size_t)n * vocab * 4), tb = al(tab.size()), mb = al((size_t)nm * words * 4);
-    const size_t ob = al((size_t)n * 4), kb = al((size_t)n * sizeof(TopkpRow));
-    float *dl = (float *)jl_scratch(ctx, 0, lb);
-    char *dw = (char *)jl_scratch(ctx, 1, 3 * rb + tb + mb);
-    float *dex = (float *)jl_scratch(ctx, 2, rb);
+    const size_t rb = al((size_t)n * vocab * 4), tb = al(h_tab.size()), ob = al((size_t)n * 4), kb = al(h_topkp.size() * sizeof(TopkpRow));
+    float *rows = (float *)jl_scratch(ctx, 0, rb);
+    char *dw = (char *)jl_scratch(ctx, 1, 3 * rb + tb + h_mask.size() * 4);
+    float *ex = (float *)jl_scratch(ctx, 2, rb);
     char *dsel = (char *)jl_scratch(ctx, 3, ob + kb + jl_argmax_scratch_bytes(n));
-    if (!dl || !dw || !dex || !dsel) return JL_ERR_OOM;
-    unsigned *dcnt = (unsigned *)dw;
-    float *dbias = (float *)(dw + rb), *dproc = (float *)(dw + 2 * rb);
-    void *dtab = dw + 3 * rb;
-    uint32_t *dmask = (uint32_t *)(dw + 3 * rb + tb);
-    int32_t *dout = (int32_t *)dsel;
-    TopkpRow *drows = (TopkpRow *)(dsel + ob);
-    void *dargs = dsel + ob + kb;
+    if (!rows || !dw || !ex || !dsel) return JL_ERR_OOM;
+    const SelectBufs b{(float *)(dw + 2 * rb), (unsigned *)dw, (float *)(dw + rb), dw + 3 * rb, h_tab.data(), (uint32_t *)(dw + 3 * rb + tb),
+                       h_mask.data(), (TopkpRow *)(dsel + ob), h_topkp.data(), ex, (int32_t *)dsel, dsel + ob + kb};
     cudaStream_t st = ctx->stream;
-    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(dl, logits, lb, cudaMemcpyHostToDevice, st));
-    const float *src = dl;
-    int64_t lds = ld;
-    if (processed) {
-        JL_CUDA_CHECK(ctx, cudaMemsetAsync(dcnt, 0, (size_t)n * vocab * 4, st));
-        JL_CUDA_CHECK(ctx, cudaMemcpyAsync(dtab, tab.data(), tab.size(), cudaMemcpyHostToDevice, st));
-        if (nm > 0) JL_CUDA_CHECK(ctx, cudaMemcpyAsync(dmask, mrows.data(), (size_t)nm * words * 4, cudaMemcpyHostToDevice, st));
-        M_CHECK(jl_launch_penalties(ctx, st, dl, ld, vocab, n, dtab, plan, dcnt, dbias, nm > 0 ? dmask : nullptr, dproc));
-        src = dproc, lds = vocab;
-    }
-    M_CHECK(jl_launch_argmax(ctx, st, src, n, vocab, (int)lds, dout, dargs));
-    std::vector<TopkpRow> hr;
-    for (int i = 0; i < n; i++)
-        if (filtered[(size_t)i]) hr.push_back(TopkpRow{i, temperatures[i], top_k ? top_k[i] : 0, top_p ? top_p[i] : 1.0f, uniforms[i]});
-    if (!hr.empty()) {
-        JL_CUDA_CHECK(ctx, cudaMemcpyAsync(drows, hr.data(), hr.size() * sizeof(TopkpRow), cudaMemcpyHostToDevice, st));
-        M_CHECK(jl_launch_sample_topkp(ctx, st, src, lds, vocab, drows, (int)hr.size(), dex, dout));
-    }
-    for (int i = 0; temperatures && i < n; i++) {
-        if (!(temperatures[i] > 0.0f) || filtered[(size_t)i]) continue;
-        softmax_sample_kernel<<<1, 256, 0, st>>>(src + (size_t)i * lds, dex + (size_t)i * vocab, vocab, temperatures[i], uniforms[i], dout + i);
-        ctx->launches++;
-        JL_CUDA_CHECK(ctx, cudaGetLastError());
-    }
-    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(out, dout, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+    JL_CUDA_CHECK(ctx, cudaMemcpy2DAsync(rows, (size_t)vocab * 4, logits, (size_t)ld * 4, (size_t)vocab * 4, n, cudaMemcpyHostToDevice, st));
+    if (s.processed()) JL_CUDA_CHECK(ctx, cudaMemsetAsync(b.cnt, 0, (size_t)n * vocab * 4, st));
+    M_CHECK(jl_launch_argmax(ctx, st, rows, n, vocab, vocab, b.next, b.argmax));
+    M_CHECK(select_pass(ctx, st, n, vocab, rows, s, b));
+    JL_CUDA_CHECK(ctx, cudaMemcpyAsync(out, b.next, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
     JL_CUDA_CHECK(ctx, cudaStreamSynchronize(st));
     return JL_OK;
 }
 
 extern "C" int jl_model_decode(jl_model *m, int n, const int32_t *sessions, const int32_t *tokens, const int32_t *positions,
                                int32_t *next_tokens, float *logits_out) {
-    return decode_impl(m, n, sessions, tokens, positions, nullptr, nullptr, next_tokens, logits_out);
+    Selection s;
+    return decode_impl(m, n, sessions, tokens, positions, next_tokens, logits_out, s);
 }
 
 extern "C" int jl_model_decode_sample(jl_model *m, int n, const int32_t *sessions, const int32_t *tokens, const int32_t *positions,
                                       const float *temperatures, const float *uniforms, int32_t *next_tokens, float *logits_out) {
-    return decode_impl(m, n, sessions, tokens, positions, temperatures, uniforms, next_tokens, logits_out);
+    Selection s{temperatures, uniforms};
+    return decode_impl(m, n, sessions, tokens, positions, next_tokens, logits_out, s);
 }
 
 extern "C" int jl_model_decode_resident(jl_model *m, int session, int32_t first_token, int start_pos, int n_new,
@@ -2200,43 +2079,44 @@ extern "C" int jl_model_last_timing(jl_model *m, double *total_ms, double *gemv_
 // arg-max and logits_out (nullable, [n_new, vocab]) gets the raw logits of each step; otherwise uniforms[i] plays
 // ThreadLocalRandom.current().nextFloat() of the i-th sample() call (:576, :594), so a caller that passes the same stream gets the same
 // tokens.
-// With `topkp` every token is sampled as by jl_model_decode_sample_topkp with (top_k, top_p), and all arguments are checked before the
-// prompt is forwarded.  `lp` (its top_n is one value for every token): the logprobs of token i go to row i of its outputs.  `gp`
-// (nullable): the penalties of every token; token i's history is the prompt and the i tokens before it.
-static int generate(jl_model *m, int session, const int32_t *prompt, int n_prompt, int n_new, float temperature, const float *uniforms,
-                    int32_t *out_tokens, float *logits_out, double *timings_ms, bool topkp = false, int top_k = 0, float top_p = 1.0f,
-                    LogprobArgs lp = LogprobArgs(), const jl_penalties *gp = nullptr) {
-    if (!m || !m->finalized || !prompt || n_prompt <= 0 || n_new <= 0 || !out_tokens || (temperature != 0.0f && !uniforms)) return JL_ERR_INVALID;
-    for (int i = 0; topkp && i < n_new; i++)
-        M_CHECK(jl_topkp_check(m->ctx, "generate", 1, m->cfg.vocab_size, &temperature, &top_k, &top_p, uniforms ? uniforms + i : nullptr,
+// `g` holds the one-row selection of every token: g.temperatures points at the temperature, g.uniforms at the uniforms of the tokens,
+// and the logprob outputs at token 0's row (token i writes row i).  All arguments are checked before the prompt is forwarded; with
+// g.topkp every token is sampled as by jl_model_decode_sample_topkp.  g.pen (nullable, its history ignored): the penalties of every
+// token; token i's history is the prompt and the i tokens before it.
+static int generate(jl_model *m, int session, const int32_t *prompt, int n_prompt, int n_new, const Selection &g, int32_t *out_tokens,
+                    float *logits_out, double *timings_ms) {
+    const float temperature = *g.temperatures;
+    if (!m || !m->finalized || !prompt || n_prompt <= 0 || n_new <= 0 || !out_tokens || (temperature != 0.0f && !g.uniforms)) return JL_ERR_INVALID;
+    for (int i = 0; g.topkp && i < n_new; i++)
+        M_CHECK(jl_topkp_check(m->ctx, "generate", 1, m->cfg.vocab_size, g.temperatures, g.top_k, g.top_p, g.uniforms ? g.uniforms + i : nullptr,
                                nullptr, nullptr));
-    M_CHECK(logprobs_check(m, "generate", 1, lp));
     // the history of token i: the prompt, then out_tokens[0, i) (generated ids come from the model, so checking the prompt's suffices)
     std::vector<int32_t> hist;
     int32_t hoff[2] = {0, n_prompt}, hprompt = n_prompt;
     jl_penalties pen = {};
-    if (gp) {
+    Selection s = g;
+    float u = temperature != 0.0f ? g.uniforms[0] : 0.0f;
+    s.uniforms = &u;
+    if (g.pen) {
         hist.assign(prompt, prompt + n_prompt);
         hist.reserve((size_t)n_prompt + n_new);
-        pen = *gp;
+        pen = *g.pen;
         pen.hist_off = hoff, pen.hist_prompt = &hprompt, pen.hist_ids = hist.data();
-        PenaltyArgs pa = penalty_args(&pen);
-        M_CHECK(penalty_check(m, "generate", 1, pa));
+        s.pen = &pen;
     }
-    auto pen_at = [&](int i) { // after out_tokens[0, i) are known
-        if (!gp) return PenaltyArgs();
-        hist.resize((size_t)n_prompt + i);
-        if (i > 0) memcpy(hist.data() + n_prompt, out_tokens, (size_t)i * 4);
-        hoff[1] = n_prompt + i;
-        pen.hist_ids = hist.data();
-        return penalty_args(&pen);
-    };
-    auto lp_at = [&](int i) { // token i: the same top_n, row i of the outputs
-        LogprobArgs a = lp;
-        a.lp = lp.lp ? lp.lp + i : nullptr;
-        a.ids = lp.ids ? lp.ids + (size_t)i * JL_MAX_LOGPROBS : nullptr;
-        a.tlp = lp.tlp ? lp.tlp + (size_t)i * JL_MAX_LOGPROBS : nullptr;
-        return a;
+    M_CHECK(select_check(m->ctx, "generate", 1, m->cfg.vocab_size, m->cfg.tp_size > 1, s));
+    auto at = [&](int i) -> Selection & { // token i, after out_tokens[0, i) are known
+        u = temperature != 0.0f ? g.uniforms[i] : 0.0f;
+        if (g.pen) {
+            hist.resize((size_t)n_prompt + i);
+            if (i > 0) memcpy(hist.data() + n_prompt, out_tokens, (size_t)i * 4);
+            hoff[1] = n_prompt + i;
+            pen.hist_ids = hist.data();
+        }
+        s.lp = g.lp ? g.lp + i : nullptr;
+        s.ids = g.ids ? g.ids + (size_t)i * JL_MAX_LOGPROBS : nullptr;
+        s.tlp = g.tlp ? g.tlp + (size_t)i * JL_MAX_LOGPROBS : nullptr;
+        return s;
     };
     std::lock_guard<std::recursive_mutex> model_lock(m->mu);
     const int V = m->cfg.vocab_size;
@@ -2244,19 +2124,16 @@ static int generate(jl_model *m, int session, const int32_t *prompt, int n_promp
     M_CHECK(jl_model_reset_session(m, session));
     M_CHECK(jl_model_batch_forward(m, session, prompt, n_prompt, 0));
     int32_t next = 0;
-    const float u0 = temperature != 0.0f ? uniforms[0] : 0.0f;
-    if (topkp)
-        M_CHECK(sample_multi_impl(m, 1, &session, &temperature, &u0, &next, nullptr, topkp_args(&top_k, &top_p), lp_at(0), pen_at(0)));
+    if (g.topkp)
+        M_CHECK(sample_multi_impl(m, 1, &session, &next, nullptr, at(0)));
     else
-        M_CHECK(jl_model_sample(m, session, temperature, u0, &next, logits_out));
+        M_CHECK(jl_model_sample(m, session, temperature, u, &next, logits_out));
     auto t1 = std::chrono::steady_clock::now();
     out_tokens[0] = next;
     for (int i = 1; i < n_new; i++) {
         const int32_t pos = n_prompt + i - 1;
-        const float u = temperature != 0.0f ? uniforms[i] : 0.0f;
         int32_t nx = 0;
-        M_CHECK(decode_impl(m, 1, &session, &next, &pos, &temperature, &u, &nx, logits_out ? logits_out + (size_t)i * V : nullptr,
-                            topkp ? topkp_args(&top_k, &top_p) : TopkpArgs(), lp_at(i), pen_at(i)));
+        M_CHECK(decode_impl(m, 1, &session, &next, &pos, &nx, logits_out ? logits_out + (size_t)i * V : nullptr, at(i)));
         next = nx;
         out_tokens[i] = next;
     }
@@ -2270,24 +2147,26 @@ static int generate(jl_model *m, int session, const int32_t *prompt, int n_promp
 
 extern "C" int jl_model_generate(jl_model *m, int session, const int32_t *prompt, int n_prompt, int n_new, int32_t *out_tokens,
                                  float *logits_out, double *timings_ms) {
-    return generate(m, session, prompt, n_prompt, n_new, 0.0f, nullptr, out_tokens, logits_out, timings_ms);
+    const float greedy = 0.0f;
+    return generate(m, session, prompt, n_prompt, n_new, Selection{&greedy}, out_tokens, logits_out, timings_ms);
 }
 
 extern "C" int jl_model_generate_sample(jl_model *m, int session, const int32_t *prompt, int n_prompt, int n_new, float temperature,
                                         const float *uniforms, int32_t *out_tokens, double *timings_ms) {
-    return generate(m, session, prompt, n_prompt, n_new, temperature, uniforms, out_tokens, nullptr, timings_ms);
+    return generate(m, session, prompt, n_prompt, n_new, Selection{&temperature, uniforms}, out_tokens, nullptr, timings_ms);
 }
 
 extern "C" int jl_model_generate_sample_topkp(jl_model *m, int session, const int32_t *prompt, int n_prompt, int n_new, float temperature,
                                               int top_k, float top_p, const float *uniforms, int32_t *out_tokens, double *timings_ms) {
-    return generate(m, session, prompt, n_prompt, n_new, temperature, uniforms, out_tokens, nullptr, timings_ms, true, top_k, top_p);
+    return generate(m, session, prompt, n_prompt, n_new, Selection{&temperature, uniforms, true, &top_k, &top_p}, out_tokens, nullptr,
+                    timings_ms);
 }
 
 extern "C" int jl_model_generate_logprobs(jl_model *m, int session, const int32_t *prompt, int n_prompt, int n_new, float temperature, int top_k,
                                           float top_p, const float *uniforms, int top_n, int32_t *out_tokens, float *lp_out, int32_t *top_ids_out,
                                           float *top_lp_out, double *timings_ms) {
-    return generate(m, session, prompt, n_prompt, n_new, temperature, uniforms, out_tokens, nullptr, timings_ms, true, top_k, top_p,
-                    logprob_args(&top_n, lp_out, top_ids_out, top_lp_out));
+    const Selection g{&temperature, uniforms, true, &top_k, &top_p, true, &top_n, lp_out, top_ids_out, top_lp_out};
+    return generate(m, session, prompt, n_prompt, n_new, g, out_tokens, nullptr, timings_ms);
 }
 
 extern "C" int jl_model_generate_penalized(jl_model *m, int session, const int32_t *prompt, int n_prompt, int n_new, float temperature,
@@ -2299,8 +2178,8 @@ extern "C" int jl_model_generate_penalized(jl_model *m, int session, const int32
     jl_penalties gp = {};
     gp.presence = &presence, gp.frequency = &frequency, gp.repetition = &repetition;
     gp.bias_off = boff, gp.bias_ids = bias_ids, gp.bias_vals = bias_vals;
-    return generate(m, session, prompt, n_prompt, n_new, temperature, uniforms, out_tokens, nullptr, timings_ms, true, top_k, top_p,
-                    logprob_args(&top_n, lp_out, top_ids_out, top_lp_out), &gp);
+    const Selection g{&temperature, uniforms, true, &top_k, &top_p, true, &top_n, lp_out, top_ids_out, top_lp_out, &gp};
+    return generate(m, session, prompt, n_prompt, n_new, g, out_tokens, nullptr, timings_ms);
 }
 
 // ---- KV persistence (KvBufferCache.KvBufferPage, core/tensor/KvBufferCache.java:121-176): the reference backs every page of a

@@ -118,6 +118,42 @@ def _penalty_struct(penalties, n):
     return native.Penalties(*[a.ctypes.data for a in arrays]), arrays
 
 
+def _select_args(n, vocab, temperatures, uniforms, top_k, top_p, logprobs, penalties, allowed):
+    """The per-row selection arguments of a decode / sample_multi call, converted once for the narrowest entry point they need:
+    (its suffix: "_constrained", "_penalized", "_logprobs", "_topkp" or "" for the plain one, its arguments before the token output,
+    those between the token output and logits_out, the TokenLogprobs it fills or None, the arrays to keep alive for the call)."""
+    t = None if temperatures is None else np.ascontiguousarray(temperatures, dtype=np.float32)
+    u = None if uniforms is None else np.ascontiguousarray(uniforms, dtype=np.float32)
+    assert (t is None or len(t) == n) and (u is None or len(u) == n)
+    if allowed is not None:
+        tier = "_constrained"
+    elif penalties is not None:
+        tier = "_penalized"
+    elif logprobs is not None:
+        tier = "_logprobs"
+    elif top_k is not None or top_p is not None:
+        tier = "_topkp"
+    else:
+        return "", (ptr(t), ptr(u)), (), None, (t, u)
+    k, p = _filter_arrays(top_k, top_p, n)
+    pre, keep = [ptr(t), ptr(k), ptr(p), ptr(u)], [t, u, k, p]
+    if tier == "_topkp":
+        return tier, pre, (), None, keep
+    tn = np.ascontiguousarray(np.broadcast_to(-1 if logprobs is None else logprobs, (n,)), dtype=np.int32)
+    lp = _logprob_arrays(n)
+    pre.append(ptr(tn))
+    keep += [tn, lp]
+    if tier != "_logprobs":
+        pen, arrays = _penalty_struct(penalties if penalties is not None else [None] * n, n)
+        pre.append(C.addressof(pen))
+        keep += [pen, arrays]
+    if tier == "_constrained":
+        n_allow, allow, allow_row = _mask_arrays(allowed, n, vocab)
+        pre += [n_allow, ptr(allow), ptr(allow_row)]
+        keep += [allow, allow_row]
+    return tier, pre, (ptr(lp.lp), ptr(lp.top_ids), ptr(lp.top_lp)), lp, keep
+
+
 class LlamaModel:
     def __init__(self, ctx, cfg, weights, working_qtype=I8, kv_dtype=F32, max_batch=256, max_sessions=1, max_context=0,
                  tp_rank=0, tp_size=1, flags=0, prefill_tensor_core=0):
@@ -280,43 +316,12 @@ class LlamaModel:
         (a bool[vocab] or packed uint32 words, DESIGN §3.18) the row is selected under; logits and logprobs stay those of the raw logits."""
         sessions = np.ascontiguousarray(sessions, dtype=np.int32)
         n = len(sessions)
-        t = None if temperatures is None else np.ascontiguousarray(temperatures, dtype=np.float32)
-        u = None if uniforms is None else np.ascontiguousarray(uniforms, dtype=np.float32)
-        assert (t is None or len(t) == n) and (u is None or len(u) == n)
         out = np.empty(n, dtype=np.int32)
         logits = np.empty((n, self.cfg["vocab"]), dtype=np.float32) if want_logits else None
-        if allowed is not None:
-            k, p = _filter_arrays(top_k, top_p, n)
-            tn = np.ascontiguousarray(np.broadcast_to(-1 if logprobs is None else logprobs, (n,)), dtype=np.int32)
-            lp = _logprob_arrays(n)
-            pen, _keep = _penalty_struct(penalties if penalties is not None else [None] * n, n)
-            n_allow, allow, allow_row = _mask_arrays(allowed, n, self.cfg["vocab"])
-            self.ctx.check(self.lib.jl_model_sample_multi_constrained(self.h, n, ptr(sessions), ptr(t), ptr(k), ptr(p), ptr(u), ptr(tn),
-                                                                      C.addressof(pen), n_allow, ptr(allow), ptr(allow_row), ptr(out),
-                                                                      ptr(lp.lp), ptr(lp.top_ids), ptr(lp.top_lp), ptr(logits)))
-            return (out, logits) if logprobs is None else (out, logits, lp)
-        if penalties is not None:
-            k, p = _filter_arrays(top_k, top_p, n)
-            tn = np.ascontiguousarray(np.broadcast_to(-1 if logprobs is None else logprobs, (n,)), dtype=np.int32)
-            lp = _logprob_arrays(n)
-            pen, _keep = _penalty_struct(penalties, n)
-            self.ctx.check(self.lib.jl_model_sample_multi_penalized(self.h, n, ptr(sessions), ptr(t), ptr(k), ptr(p), ptr(u), ptr(tn),
-                                                                    C.addressof(pen), ptr(out), ptr(lp.lp), ptr(lp.top_ids), ptr(lp.top_lp),
-                                                                    ptr(logits)))
-            return (out, logits) if logprobs is None else (out, logits, lp)
-        if logprobs is not None:
-            k, p = _filter_arrays(top_k, top_p, n)
-            tn = np.ascontiguousarray(np.broadcast_to(logprobs, (n,)), dtype=np.int32)
-            lp = _logprob_arrays(n)
-            self.ctx.check(self.lib.jl_model_sample_multi_logprobs(self.h, n, ptr(sessions), ptr(t), ptr(k), ptr(p), ptr(u), ptr(tn), ptr(out),
-                                                                   ptr(lp.lp), ptr(lp.top_ids), ptr(lp.top_lp), ptr(logits)))
-            return out, logits, lp
-        if top_k is None and top_p is None:
-            self.ctx.check(self.lib.jl_model_sample_multi(self.h, n, ptr(sessions), ptr(t), ptr(u), ptr(out), ptr(logits)))
-        else:
-            k, p = _filter_arrays(top_k, top_p, n)
-            self.ctx.check(self.lib.jl_model_sample_multi_topkp(self.h, n, ptr(sessions), ptr(t), ptr(k), ptr(p), ptr(u), ptr(out), ptr(logits)))
-        return out, logits
+        tier, pre, post, lp, _keep = _select_args(n, self.cfg["vocab"], temperatures, uniforms, top_k, top_p, logprobs, penalties, allowed)
+        call = getattr(self.lib, "jl_model_sample_multi" + tier)
+        self.ctx.check(call(self.h, n, ptr(sessions), *pre, ptr(out), *post, ptr(logits)))
+        return (out, logits) if logprobs is None else (out, logits, lp)
 
     def decode(self, tokens, positions, sessions=None, want_logits=False, temperatures=None, uniforms=None, top_k=None, top_p=None,
                logprobs=None, penalties=None, allowed=None):
@@ -332,57 +337,14 @@ class LlamaModel:
         sessions = np.arange(n, dtype=np.int32) if sessions is None else np.ascontiguousarray(sessions, dtype=np.int32)
         nxt = np.empty(n, dtype=np.int32)
         logits = np.empty((n, self.cfg["vocab"]), dtype=np.float32) if want_logits else None
-        if allowed is not None:
-            t = None if temperatures is None else np.ascontiguousarray(temperatures, dtype=np.float32)
-            u = None if uniforms is None else np.ascontiguousarray(uniforms, dtype=np.float32)
-            assert (t is None or len(t) == n) and (u is None or len(u) == n)
-            k, p = _filter_arrays(top_k, top_p, n)
-            tn = np.ascontiguousarray(np.broadcast_to(-1 if logprobs is None else logprobs, (n,)), dtype=np.int32)
-            lp = _logprob_arrays(n)
-            pen, _keep = _penalty_struct(penalties if penalties is not None else [None] * n, n)
-            n_allow, allow, allow_row = _mask_arrays(allowed, n, self.cfg["vocab"])
-            self.ctx.check(self.lib.jl_model_decode_constrained(self.h, n, ptr(sessions), ptr(tokens), ptr(positions), ptr(t), ptr(k), ptr(p),
-                                                                ptr(u), ptr(tn), C.addressof(pen), n_allow, ptr(allow), ptr(allow_row), ptr(nxt),
-                                                                ptr(lp.lp), ptr(lp.top_ids), ptr(lp.top_lp), ptr(logits)))
-            return (nxt, logits) if logprobs is None else (nxt, logits, lp)
-        if penalties is not None:
-            t = None if temperatures is None else np.ascontiguousarray(temperatures, dtype=np.float32)
-            u = None if uniforms is None else np.ascontiguousarray(uniforms, dtype=np.float32)
-            assert (t is None or len(t) == n) and (u is None or len(u) == n)
-            k, p = _filter_arrays(top_k, top_p, n)
-            tn = np.ascontiguousarray(np.broadcast_to(-1 if logprobs is None else logprobs, (n,)), dtype=np.int32)
-            lp = _logprob_arrays(n)
-            pen, _keep = _penalty_struct(penalties, n)
-            self.ctx.check(self.lib.jl_model_decode_penalized(self.h, n, ptr(sessions), ptr(tokens), ptr(positions), ptr(t), ptr(k), ptr(p), ptr(u),
-                                                              ptr(tn), C.addressof(pen), ptr(nxt), ptr(lp.lp), ptr(lp.top_ids), ptr(lp.top_lp),
-                                                              ptr(logits)))
-            return (nxt, logits) if logprobs is None else (nxt, logits, lp)
-        if logprobs is not None:
-            t = None if temperatures is None else np.ascontiguousarray(temperatures, dtype=np.float32)
-            u = None if uniforms is None else np.ascontiguousarray(uniforms, dtype=np.float32)
-            assert (t is None or len(t) == n) and (u is None or len(u) == n)
-            k, p = _filter_arrays(top_k, top_p, n)
-            tn = np.ascontiguousarray(np.broadcast_to(logprobs, (n,)), dtype=np.int32)
-            lp = _logprob_arrays(n)
-            self.ctx.check(self.lib.jl_model_decode_logprobs(self.h, n, ptr(sessions), ptr(tokens), ptr(positions), ptr(t), ptr(k), ptr(p), ptr(u),
-                                                             ptr(tn), ptr(nxt), ptr(lp.lp), ptr(lp.top_ids), ptr(lp.top_lp), ptr(logits)))
-            return nxt, logits, lp
-        if top_k is not None or top_p is not None:
-            t = None if temperatures is None else np.ascontiguousarray(temperatures, dtype=np.float32)
-            u = None if uniforms is None else np.ascontiguousarray(uniforms, dtype=np.float32)
-            assert (t is None or len(t) == n) and (u is None or len(u) == n)
-            k, p = _filter_arrays(top_k, top_p, n)
-            self.ctx.check(self.lib.jl_model_decode_sample_topkp(self.h, n, ptr(sessions), ptr(tokens), ptr(positions), ptr(t), ptr(k), ptr(p),
-                                                                 ptr(u), ptr(nxt), ptr(logits)))
-        elif temperatures is None:
-            self.ctx.check(self.lib.jl_model_decode(self.h, n, ptr(sessions), ptr(tokens), ptr(positions), ptr(nxt), ptr(logits)))
+        tier, pre, post, lp, _keep = _select_args(n, self.cfg["vocab"], temperatures, uniforms, top_k, top_p, logprobs, penalties, allowed)
+        rows = (self.h, n, ptr(sessions), ptr(tokens), ptr(positions))
+        if not tier and temperatures is None:
+            self.ctx.check(self.lib.jl_model_decode(*rows, ptr(nxt), ptr(logits)))
         else:
-            t = np.ascontiguousarray(temperatures, dtype=np.float32)
-            u = np.ascontiguousarray(uniforms, dtype=np.float32)
-            assert len(t) == n and len(u) == n
-            self.ctx.check(self.lib.jl_model_decode_sample(self.h, n, ptr(sessions), ptr(tokens), ptr(positions), ptr(t), ptr(u), ptr(nxt),
-                                                           ptr(logits)))
-        return nxt, logits
+            call = getattr(self.lib, "jl_model_decode" + ("_sample" + tier if tier in ("", "_topkp") else tier))
+            self.ctx.check(call(*rows, *pre, ptr(nxt), *post, ptr(logits)))
+        return (nxt, logits) if logprobs is None else (nxt, logits, lp)
 
     def score_multi(self, segments, top_n=0):
         """batch_forward_multi that also scores the tokens (DESIGN §3.13): segments = [(session, tokens, start_pos), ...].  Returns one
@@ -425,30 +387,23 @@ class LlamaModel:
         u = np.ascontiguousarray(uniforms, dtype=np.float32)
         assert len(u) >= n_new
         out = np.empty(n_new, dtype=np.int32)
+        lp = _logprob_arrays(n_new)
+        head = (self.h, session, ptr(prompt), len(prompt), n_new, C.c_float(temperature))
+        filt = (int(top_k or 0), C.c_float(1.0 if top_p is None else top_p), ptr(u))
+        lp_out = (ptr(lp.lp), ptr(lp.top_ids), ptr(lp.top_lp))
+        top_n = -1 if logprobs is None else int(logprobs)
         if penalties is not None:
             q = RowPenalty(*penalties)
             bi, bv = _bias_pairs(q.logit_bias)
-            lp = _logprob_arrays(n_new)
-            self.ctx.check(self.lib.jl_model_generate_penalized(self.h, session, ptr(prompt), len(prompt), n_new, C.c_float(temperature),
-                                                                int(top_k or 0), C.c_float(1.0 if top_p is None else top_p), ptr(u),
-                                                                -1 if logprobs is None else int(logprobs), C.c_float(q.presence),
-                                                                C.c_float(q.frequency), C.c_float(q.repetition), len(bi), ptr(bi), ptr(bv),
-                                                                ptr(out), ptr(lp.lp), ptr(lp.top_ids), ptr(lp.top_lp), None))
-            return out if logprobs is None else (out, lp)
-        if logprobs is not None:
-            lp = _logprob_arrays(n_new)
-            self.ctx.check(self.lib.jl_model_generate_logprobs(self.h, session, ptr(prompt), len(prompt), n_new, C.c_float(temperature),
-                                                               int(top_k or 0), C.c_float(1.0 if top_p is None else top_p), ptr(u), int(logprobs),
-                                                               ptr(out), ptr(lp.lp), ptr(lp.top_ids), ptr(lp.top_lp), None))
-            return out, lp
-        if top_k is None and top_p is None:
-            self.ctx.check(self.lib.jl_model_generate_sample(self.h, session, ptr(prompt), len(prompt), n_new, C.c_float(temperature), ptr(u),
-                                                             ptr(out), None))
+            self.ctx.check(self.lib.jl_model_generate_penalized(*head, *filt, top_n, C.c_float(q.presence), C.c_float(q.frequency),
+                                                                C.c_float(q.repetition), len(bi), ptr(bi), ptr(bv), ptr(out), *lp_out, None))
+        elif logprobs is not None:
+            self.ctx.check(self.lib.jl_model_generate_logprobs(*head, *filt, top_n, ptr(out), *lp_out, None))
+        elif top_k is None and top_p is None:
+            self.ctx.check(self.lib.jl_model_generate_sample(*head, ptr(u), ptr(out), None))
         else:
-            self.ctx.check(self.lib.jl_model_generate_sample_topkp(self.h, session, ptr(prompt), len(prompt), n_new, C.c_float(temperature),
-                                                                   int(top_k or 0), C.c_float(1.0 if top_p is None else top_p), ptr(u),
-                                                                   ptr(out), None))
-        return out
+            self.ctx.check(self.lib.jl_model_generate_sample_topkp(*head, *filt, ptr(out), None))
+        return out if logprobs is None else (out, lp)
 
     def kv_save(self, directory, session_name, session=0):
         """KvBufferCache.KvBufferPage persistence: <directory>/<session_name>-L<l>C<c>.page files; returns the page count."""
